@@ -2,7 +2,7 @@
 """Benchmark of the CTSD-3.5 diffusion-forcing denoise step (BASELINE.json metric:
 denoise-steps/sec, 6 views x 16 frames, CFG on).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo (sm_100a kernels)
+  python bench.py --gpus N --steps K --warmup W            # this repo (sm_90a kernels)
   python bench.py --impl reference --steps K --warmup W    # reference semantics on host CPU
 
 One "step" = one iteration of StreamingCrossviewTemporalSD.inference_pipeline's loop
@@ -56,8 +56,9 @@ def peaks():
         with open(path) as f:
             d = json.load(f)
         _PEAKS.update(d)
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs"), "measured"
-    return 1400.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs"), "measured"
+    # NVIDIA H100 SXM data sheet (700 W): dense BF16 / FP16 and HBM3 bandwidth
+    return 989.0, 3350.0, "datasheet"
 
 
 _PEAKS = {}
@@ -174,6 +175,9 @@ def run_native(args):
     if world != args.gpus:
         if world == 1 and args.gpus > 1:
             raise SystemExit("launch with torch.distributed.run for --gpus > 1")
+    if args.dump_outputs and world > 1:
+        # each rank holds only its CFG branch / frame shard of the latents
+        raise SystemExit("--dump-outputs records the unsharded step: run it with --gpus 1")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -271,6 +275,8 @@ def run_native(args):
     sync()
     prof = ops.profile_end()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, latents)
     ms = e0.elapsed_time(e1) / args.steps
     if world > 1:
         t = torch.tensor([ms], device=dev)
@@ -315,20 +321,8 @@ def run_native(args):
         a[2] += p_["flops"]
     dom_key, dom = max(by_shape.items(), key=lambda kv: kv[1][1])
     achieved = dom[2] / (dom[1] * 1e-3) / 1e12
-    # DRAM bytes per launch of that kernel: NOT measurable inside this run (no counters without
-    # ncu); looked up in profiles/ncu_traffic.json, which records, per (M,N,K,epilogue,dtype),
-    # dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full` launch and the
-    # capture file it came from.  null when no capture of this kernel shape is committed.
+    # DRAM bytes per launch of that kernel are not measurable inside this run (no counters)
     traffic, traffic_src = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            for row in json.load(f)["kernels"]:
-                if tuple(row["shape"]) == dom_key[0] and row["epilogue"] == dom_key[1] and \
-                        row.get("dtype", args.dtype) == args.dtype:
-                    traffic = row["dram_read_bytes"] + row["dram_write_bytes"]
-                    traffic_src = row["capture"]
-    except Exception:  # noqa: BLE001
-        pass
     scale = 1.0 if not args.small else None
     line = {
         "metric": METRIC, "value": 1000.0 / ms, "unit": "steps/s",
@@ -349,7 +343,7 @@ def run_native(args):
             "bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
             "frac": (achieved / peak_tf) if achieved else None, "traffic": traffic,
             "traffic_source": traffic_src,
-            "kernel": "gemm2_tcgen05_kernel M=%d N=%d K=%d epilogue=%d (CUDA events around "
+            "kernel": "gemm_wgmma_kernel M=%d N=%d K=%d epilogue=%d (CUDA events around "
                       "each of its %d launches in the timed steps)" % (dom_key[0] + (dom_key[1], dom[0])),
             "algorithmic_flops_per_launch": dom[2] / dom[0],
             "kernel_share_of_step": dom[1] / (ms * args.steps),
@@ -427,6 +421,16 @@ def run_native(args):
         line["cpu_baseline"] = cpu_baseline(budget_s=args.cpu_budget, small=args.small)
     print(json.dumps(line), flush=True)
     _leave(world)
+
+
+def dump_outputs(out_dir, latents):
+    """What the timed loop computed: the latents its last step left behind, the array a caller
+    of `denoise_step` receives (11 MB in float32 at the north-star shape; single GPU only).
+    Inputs and weights are seeded, so two builds run with the same arguments can be compared
+    output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "latents.npy"), latents.float().cpu().numpy())
 
 
 def _leave(world):
@@ -631,7 +635,12 @@ def main():
                     help="skip streaming_e2e / workloads / eager_gpu_baseline / other dtype")
     ap.add_argument("--profile-dump", default=None,
                     help="write per-shape GEMM timing of the timed steps to this JSON")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the latents of the last step to "
+                         "DIR/latents.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "native":
+        ap.error("--dump-outputs records the native step; it has no meaning with --impl reference")
     if args.impl == "reference":
         run_reference(args)
     else:

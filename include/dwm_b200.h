@@ -1,5 +1,5 @@
 /*
- * dwm_b200 — C ABI of the B200-native (sm_100a) kernels behind OpenDWM's CTSD
+ * dwm_b200 — C ABI of the H100-native (sm_90a) kernels behind OpenDWM's CTSD
  * denoising hot path.
  *
  * The reference (SenseTime-FVG/OpenDWM) has no C/FFI interface of its own: its
@@ -16,7 +16,7 @@
  *    allocated here.  Launches are asynchronous on `stream`.
  *  - 16-bit activations/weights are bf16 (DWM_BF16) or fp16 (DWM_F16);
  *    biases, norm weights, modulation vectors, residual streams are fp32.
- *  - there is NO CPU fallback: calling these without a Blackwell GPU fails.
+ *  - there is NO CPU fallback: calling these without a Hopper (sm_90a) GPU fails.
  */
 #ifndef DWM_B200_H_
 #define DWM_B200_H_
@@ -33,7 +33,7 @@ typedef void* dwm_stream_t; /* cudaStream_t */
 enum dwm_dtype { DWM_BF16 = 0, DWM_F16 = 1, DWM_F32 = 2 };
 enum dwm_act { DWM_ACT_NONE = 0, DWM_ACT_GELU_TANH = 1, DWM_ACT_GELU_ERF = 2, DWM_ACT_SILU = 3, DWM_ACT_RELU = 4 };
 
-/* Epilogues of dwm_b200_linear (all fused into the tcgen05 GEMM kernel). */
+/* Epilogues of dwm_b200_linear (all fused into the wgmma GEMM kernel). */
 enum dwm_epilogue {
   /* out16[r(m), n] = act(acc + bias[n]) */
   DWM_EPI_STORE = 0,
@@ -103,20 +103,20 @@ typedef struct dwm_linear_args {
 const char* dwm_b200_version(void);
 const char* dwm_b200_last_error(void);
 /* Runtime switches (no reference counterpart; they select between kernels that must agree,
- * which tests/ use for kernel-variant parity): "gemm_2cta" = 1 routes dwm_b200_linear (M >= 512) to the 2-CTA
- * cta_group::2 kernel, 0 to the 1-CTA kernel (default: env DWM_GEMM_2CTA, else 1);
+ * which tests/ use for kernel-variant parity): "gemm_2cta" = 1 routes dwm_b200_linear (M >= 512)
+ * to the kernel for clusters of two CTAs that share each weight tile by TMA multicast, 0 to the
+ * 1-CTA kernel (default: env DWM_GEMM_2CTA, else 1);
  * "attn_tc" routes eligible head_dim-64 attention (contiguous sequences; gathered sequences of
- * whole `inner`-token units with an optional unit mask): 2 = tcgen05 kernel with two
- * co-resident CTAs per SM and O in TMEM (default), 0 = mma.sync kernel, -1 = re-read env
- * DWM_ATTN_TC / DWM_ATTN_LEGACY;
+ * whole `inner`-token units with an optional unit mask): >= 1 = wgmma kernel (default), 0 =
+ * mma.sync kernel, -1 = re-read env DWM_ATTN_TC / DWM_ATTN_LEGACY;
  * "ln_staged" = 1 (default) runs large LayerNorms through the bulk-copy staged kernel, 0
  * keeps the register-resident kernel;
- * "resid_tma" = 1 (default) stages the fp32 residual tile of DWM_EPI_RESID through shared
- * memory with TMA loads and stores (2-CTA kernel, plain [M,N] residual), 0 keeps the
- * register / transposing epilogue;
- * "gemm_bn" = 0 (default) picks the RESID tile width by wave efficiency, 128 / 256 force it;
- * "conv_2cta" = 1 (default) runs convolutions with >= 2 pixel tiles per SM on the
- * cta_group::2 kernel, 0 on the 1-CTA kernel; "conv_halo" = 1 (default) routes kw = 3,
+ * "resid_tma" = 1 (default) has the TMA unit prefetch the residual / blend rows of a
+ * DWM_EPI_RESID tile into L2 while its MMAs run, 0 leaves them to the epilogue's loads;
+ * "gemm_bn" = 0 (default) picks the GEMM tile width (128 or 256 columns) by wave
+ * efficiency, 128 / 256 force it (GEGLU always uses 256);
+ * "conv_2cta" = 1 (default) runs convolutions with >= 2 pixel tiles per SM on clusters of two
+ * CTAs sharing each weight slice, 0 on the 1-CTA kernel; "conv_halo" = 1 (default) routes kw = 3,
  * W >= 128, C_out-tile <= 128 convolutions to the halo-row kernel (one load of a 130-pixel
  * row segment serves the three dw taps), 0 to the per-tap kernels. */
 int dwm_b200_set_option(const char* name, int value);
@@ -255,7 +255,7 @@ int dwm_b200_euler_step_by_indices(const float* model_output, float* sample, int
                                    int n_sigmas, int round_dtype, dwm_stream_t stream);
 
 /* ---- convolution -------------------------------------------------------------------- */
-/* im2col-free convolution (implicit GEMM on tcgen05) over channels-last activations:
+/* im2col-free convolution (implicit GEMM on wgmma) over channels-last activations:
  *   x      16-bit [nb, tp, h, w, c_in]   (tp includes the KT-1 leading causal frames)
  *   weight 16-bit [kt*kh*kw, c_out, c_in] (tap-major: tap = (dt*kh + dh)*kw + dw)
  *   out    rows = nb*(tp-kt+1)*h*w pixels, c_out columns (channels-last), pitch ldo

@@ -1,4 +1,4 @@
-"""Builds opendwm_b200/libdwm_b200.so (sm_100a) in-tree with nvcc.
+"""Builds opendwm_b200/libdwm_b200.so (sm_90a) in-tree with nvcc.
 
 Usage: python -m opendwm_b200.build [--debug-wait] [--force]
 
@@ -20,7 +20,7 @@ LIB = os.path.join(HERE, "libdwm_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
     "-std=c++17", "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
 ]
@@ -77,7 +77,7 @@ def build(debug_wait=False, force=False, verbose=False):
             futs.append(ex.submit(_compile, s, obj, flags, log))
         for f in futs:
             objs.append(f.result())
-    cmd = ["nvcc", "-shared", "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = ["nvcc", "-shared", "-gencode", "arch=compute_90a,code=sm_90a",
            "-o", LIB, *objs]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

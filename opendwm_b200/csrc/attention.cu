@@ -12,15 +12,16 @@
 // of the fused [rows, 3*D] q|k|v buffer written by the QKNORM GEMM epilogue.
 //
 // Flash-style streaming softmax, fp32 statistics; QK^T and PV run on mma.sync
-// m16n8k16 (tiles here are 16..602 long and the op is <4% of the step's FLOPs; the
-// tcgen05 pipeline is reserved for the projections/FFNs that dominate).
+// m16n8k16.  The long contiguous and gathered-unit sequences go to the wgmma kernel of
+// attention_wgmma.cu; this kernel takes the rest (pointwise temporal, separate K,V, short
+// sequences).
 #include <stdlib.h>
 
 #include "common.cuh"
 #include "../../include/dwm_b200.h"
 
 namespace dwm {
-extern int g_attn_tc;   // -1: from env, 0: mma.sync kernel only, >= 1: attention_tc2.cu when eligible (gemm.cu)
+extern int g_attn_tc;   // -1: from env, 0: mma.sync kernel only, >= 1: attention_wgmma.cu when eligible (gemm.cu)
 
 constexpr int HD = 64;
 
@@ -334,11 +335,11 @@ static int launch_attn(const AttnParams& p, cudaStream_t s) {
   return 0;
 }
 
-// attention_tc2.cu (tcgen05: two co-resident CTAs per SM, O in TMEM): contiguous sequences
-// and gathered unit sequences (cross-view / temporal row-wise, optional unit mask)
+// attention_wgmma.cu: contiguous sequences and gathered unit sequences (cross-view /
+// temporal row-wise, optional unit mask)
 bool attn_tc_eligible(const dwm_attention_args* a);
 bool attn_tcg_eligible(const dwm_attention_args* a);
-int attn_tc2_launch(const dwm_attention_args* a, cudaStream_t s);
+int attn_wgmma_launch(const dwm_attention_args* a, cudaStream_t s);
 int attn_tcg_launch(const dwm_attention_args* a, cudaStream_t s);
 
 }  // namespace dwm
@@ -360,13 +361,13 @@ extern "C" int dwm_b200_attention(const dwm_attention_args* a, dwm_stream_t stre
   if (a->mask) DWM_REQUIRE(a->mask_div > 0 && a->n_outer > 0, "dwm_b200_attention: mask needs mask_div, n_outer");
   {
     // contiguous sequences (joint / dual attention) and gathered unit sequences (cross-view /
-    // temporal row-wise) run on tcgen05 + TMEM; the rest (pointwise temporal, separate K,V,
+    // temporal row-wise) run on the wgmma kernel; the rest (pointwise temporal, separate K,V,
     // short sequences) on the mma.sync kernel below
-    if (g_attn_tc < 0) {   // env DWM_ATTN_TC = 0 | 2 (DWM_ATTN_LEGACY: same as 0); default 2
+    if (g_attn_tc < 0) {   // env DWM_ATTN_TC = 0 | 1 (DWM_ATTN_LEGACY: same as 0); default 1
       const char* e = getenv("DWM_ATTN_TC");
-      g_attn_tc = getenv("DWM_ATTN_LEGACY") != nullptr ? 0 : (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 2;
+      g_attn_tc = getenv("DWM_ATTN_LEGACY") != nullptr ? 0 : (e && e[0] >= '0' && e[0] <= '1') ? e[0] - '0' : 1;
     }
-    if (g_attn_tc >= 1 && attn_tc_eligible(a)) return attn_tc2_launch(a, reinterpret_cast<cudaStream_t>(stream));
+    if (g_attn_tc >= 1 && attn_tc_eligible(a)) return attn_wgmma_launch(a, reinterpret_cast<cudaStream_t>(stream));
     if (g_attn_tc >= 1 && attn_tcg_eligible(a)) return attn_tcg_launch(a, reinterpret_cast<cudaStream_t>(stream));
   }
   const long long groups = static_cast<long long>(a->group_dims[0]) * a->group_dims[1] * a->group_dims[2];

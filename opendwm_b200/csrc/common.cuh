@@ -1,8 +1,8 @@
-// Shared device/host helpers for the dwm_b200 sm_100a kernels.
+// Shared device/host helpers for the dwm_b200 sm_90a kernels.
 //
-// Everything here is raw PTX for Blackwell (tcgen05 / TMEM / TMA / mbarrier).
-// No CUTLASS/CuTe is included; the bit layouts of the UMMA shared-memory
-// descriptor and instruction descriptor follow the PTX ISA tables.
+// Everything here is raw PTX for Hopper (wgmma / TMA / mbarrier).
+// No CUTLASS/CuTe is included; the bit layout of the wgmma shared-memory
+// descriptor follows the PTX ISA tables.
 #pragma once
 
 #include <cuda.h>
@@ -158,97 +158,74 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint64_t* bar,
       : "memory");
 }
 
-// ---- tcgen05 / TMEM ---------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// ---- clusters of two CTAs ----------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
 }
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// Whole warp must execute.  ncols: power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+  return r;
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]^T   (both operands K-major), one thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
+// 2-D tile load written to the same shared-memory offset of every CTA in `mask`; each
+// destination's mbarrier at the offset of `bar` receives the transaction bytes
+__device__ __forceinline__ void tma_load_2d_mc(const CUtensorMap* m, uint64_t* bar, void* smem, int32_t c0,
+                                               int32_t c1, uint16_t mask, uint64_t cache_hint) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      ".L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5, %6;"
       :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      : "r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+        "h"(mask), "l"(cache_hint)
       : "memory");
-}
-// Makes the mbarrier track completion of all prior tcgen05.mma of this thread.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread t of the warp receives lane (base+t).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-      " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31},"
-      "[%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32"
-      "[%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16,"
-      " %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
 }
 
-// UMMA shared-memory matrix descriptor for a K-major operand tile written by
-// TMA with 128-byte swizzle: rows are 128 B apart, 8-row groups 1024 B apart.
-//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4 (=1, unused for SW128 K-major)
-//   [32,46) stride byte offset >> 4   [46,48) descriptor version (1 on sm_100)
-//   [61,64) layout type (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// ---- wgmma (Hopper warpgroup MMA) -----------------------------------------------
+// Shared-memory matrix descriptor for a K-major operand tile written by TMA with 128-byte
+// swizzle: rows are 128 B apart, 8-row groups 1024 B apart.
+//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4 (unused for SW128 K-major)
+//   [32,46) stride byte offset >> 4   [49,52) base offset (0: tiles are 1024-byte aligned)
+//   [62,64) layout type (1 = SWIZZLE_128B)
+// Advancing 16 elements (32 B) along K inside the swizzle atom adds 2 to the start field.
+// The 128-byte swizzle phase follows the absolute shared-memory address bits [7:9], exactly as
+// TMA wrote the tile, so a row-shifted view (start k x 128 B past a 1024-byte boundary) needs
+// no base offset: the field stays 0.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor, kind::f16, fp32 accumulate, both operands K-major.
-//   [4,6) D format (1 = f32)  [7,10) A format  [10,13) B format (0 = f16, 1 = bf16)
-//   [15] A major  [16] B major (0 = K)  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc(int m, int n, int ab_fmt) {
-  return (1u << 4) | (static_cast<uint32_t>(ab_fmt) << 7) | (static_cast<uint32_t>(ab_fmt) << 10) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
+// Orders register accesses of the accumulators before the next wgmma of this warpgroup.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Keeps the compiler from moving accumulator reads / writes across wgmma_fence / wgmma_wait.
+template <int N>
+__device__ __forceinline__ void fence_operands(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Register re-partition between warpgroups (whole warpgroup executes).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ---- numerics ---------------------------------------------------------------
 __device__ __forceinline__ float gelu_erf(float x) {
@@ -268,7 +245,6 @@ template <typename T>
 struct Cvt;
 template <>
 struct Cvt<__nv_bfloat16> {
-  static constexpr int kUmmaFmt = 1;
   __device__ static __forceinline__ uint32_t pack2(float a, float b) {
     __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&v);
@@ -282,7 +258,6 @@ struct Cvt<__nv_bfloat16> {
 };
 template <>
 struct Cvt<__half> {
-  static constexpr int kUmmaFmt = 0;
   __device__ static __forceinline__ uint32_t pack2(float a, float b) {
     __half2 v = __floats2half2_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&v);

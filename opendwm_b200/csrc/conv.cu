@@ -1,14 +1,15 @@
-// im2col-free convolution on tcgen05 (sm_100a): implicit GEMM over channels-last
+// im2col-free convolution on wgmma (sm_90a): implicit GEMM over channels-last
 // activations.  For every filter tap (dt, dh, dw) the producer TMA-loads the SHIFTED
 // bw x bh pixel patch (5-D tensor map over [NB, TP, H, W, C]; spatial zero padding is the
-// TMA out-of-bounds fill) plus that tap's [C_out, C_in] weight slice, and the MMA warp
-// accumulates all taps x channel blocks into one TMEM accumulator.  No column matrix is
-// ever materialised.  Temporal padding is NOT implicit: the caller provides TP = T_out +
-// KT - 1 frames (causal convolutions keep their cache / replicated frames in front).
+// TMA out-of-bounds fill) plus that tap's [C_out, C_in] weight slice, and the two consumer
+// warpgroups accumulate all taps x channel blocks into one register accumulator (64 pixel
+// rows each).  No column matrix is ever materialised.  Temporal padding is NOT implicit: the
+// caller provides TP = T_out + KT - 1 frames (causal convolutions keep their cache /
+// replicated frames in front).
 //
 // Used by: CogVideoX causal conv3d (3x3x3), its per-frame upsampler conv2d (1x3x3), and
 // the T2I-adapter 3x3 convs.  Epilogues are the GEMM ones (bias/act store, fp32 residual).
-#include "cta_pair.cuh"
+#include "gemm_epilogue.cuh"
 
 namespace dwm {
 
@@ -23,459 +24,149 @@ struct ConvGeom {
   int c_in, c_out;
 };
 
-template <typename T, int EPI, int CBN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-    conv_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                        const ConvGeom g, EpiParams p) {
-  constexpr int B_BYTES = CBN * BK * 2;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + CV_STAGES * CV_A_BYTES;
-  float4* epi_stage = reinterpret_cast<float4*>(smem + CV_STAGES * (CV_A_BYTES + B_BYTES));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + CV_STAGES * (CV_A_BYTES + B_BYTES) + EPI_STAGE_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + CV_STAGES;
-  uint64_t* tfull_bar = bars + 2 * CV_STAGES;
-  uint64_t* tempty_bar = bars + 2 * CV_STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * CV_STAGES + 4);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_blocks = (g.c_out + CBN - 1) / CBN;
-  const int c_blocks = (g.c_in + BK - 1) / BK;
-  const int taps = g.kt * g.kh * g.kw;
-  const int k_iters = taps * c_blocks;
-  const int tiles_per_frame = g.tiles_w * g.tiles_h;
-  const long long num_tiles = static_cast<long long>(g.nb) * g.t_out * tiles_per_frame * n_blocks;
-  const uint32_t stage_tx = static_cast<uint32_t>(g.bw * g.bh * BK * 2 + B_BYTES);
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_x);
-    tma_prefetch_desc(&tmap_w);
-    for (int s = 0; s < CV_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], EPI_WARPS); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  // tile -> (n_blk fastest, then w tile, h tile, frame, volume)
-  auto decode = [&](long long tile, int& n_blk, int& w0, int& h0, int& t, int& nb) {
-    n_blk = static_cast<int>(tile % n_blocks);
-    long long r = tile / n_blocks;
-    w0 = static_cast<int>(r % g.tiles_w) * g.bw; r /= g.tiles_w;
-    h0 = static_cast<int>(r % g.tiles_h) * g.bh; r /= g.tiles_h;
-    t = static_cast<int>(r % g.t_out);
-    nb = static_cast<int>(r / g.t_out);
-  };
-
-  if (warp == 0) {
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int n_blk, w0, h0, t, nb;
-        decode(tile, n_blk, w0, h0, t, nb);
-        for (int tap = 0; tap < taps; ++tap) {
-          const int dw = tap % g.kw, dh = (tap / g.kw) % g.kh, dt = tap / (g.kw * g.kh);
-          for (int cb = 0; cb < c_blocks; ++cb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_expect_tx(&full_bar[stage], stage_tx);
-            tma_load_5d(&tmap_x, &full_bar[stage], smem_a + stage * CV_A_BYTES, cb * BK,
-                        w0 + dw - g.kw / 2, h0 + dh - g.kh / 2, t + dt, nb, kEvictNormal);
-            tma_load_2d(&tmap_w, &full_bar[stage], smem_b + stage * B_BYTES, cb * BK,
-                        tap * g.c_out + n_blk * CBN, kEvictLast);
-            if (++stage == CV_STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc(BM, CBN, Cvt<T>::kUmmaFmt);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * CBN;
-        for (int ki = 0; ki < k_iters; ++ki) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t da = umma_desc_sw128(smem_u32(smem_a + stage * CV_A_BYTES));
-          const uint64_t db = umma_desc_sw128(smem_u32(smem_b + stage * B_BYTES));
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k)
-            umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (ki | k) ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == CV_STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull_bar[as]);
-      }
-    }
-    __syncwarp();
-  } else {
-    const int quarter = warp & 3;
-    int it = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      int n_blk, w0, h0, t, nb;
-      decode(tile, n_blk, w0, h0, t, nb);
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + as * CBN + (static_cast<uint32_t>(quarter * 32) << 16);
-      TileGeom tg;
-      tg.bw = g.bw; tg.rows = g.bw * g.bh; tg.w_lim = g.w - w0; tg.h_lim = g.h - h0; tg.img_w = g.w;
-      tg.tile_cols = CBN;
-      const int m_base = ((nb * g.t_out + t) * g.h + h0) * g.w + w0;
-      drain_tile<T, EPI>(taddr, epi_stage + (warp - 2) * 256, m_base, quarter * 32, 0, n_blk * CBN, g.c_out, p,
-                         lane, (warp - 2) >> 2, tg);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[as]);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// cta_group::2 variant: a cluster of two CTAs computes TWO pixel tiles (M = 256) x CBN output
-// channels.  Each CTA stages its own shifted pixel patch (A, 128 rows) and HALF of the tap's
-// weight slice, so per MMA step an SM reads 4 KB + CBN/2 x 32 B of shared memory: at
-// C_out = 128 that is 96 B/clk instead of the 128 B/clk that made the 1-CTA kernel shared-
-// memory bound (tensor pipe 47 %, profiles/r01_ncu_kernels_summary.txt); at C_out = 256 it is
-// 64 instead of 96 B/clk (less energy per FLOP).  Protocol = gemm2.cu.  An odd tile count gives
-// the last pair a dummy second tile: its loads are out of bounds (zero fill) and its rows are
-// never stored.
-constexpr int CV2_STAGES = 5;
-
-template <typename T, int EPI, int CBN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-    conv2_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                         const ConvGeom g, EpiParams p) {
-  constexpr int B_BYTES = (CBN / 2) * BK * 2;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + CV2_STAGES * CV_A_BYTES;
-  float4* epi_stage = reinterpret_cast<float4*>(smem + CV2_STAGES * (CV_A_BYTES + B_BYTES));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + CV2_STAGES * (CV_A_BYTES + B_BYTES) + EPI_STAGE_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + CV2_STAGES;
-  uint64_t* tfull_bar = bars + 2 * CV2_STAGES;
-  uint64_t* tempty_bar = bars + 2 * CV2_STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * CV2_STAGES + 4);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int cluster_id = blockIdx.x >> 1;
-  const int n_clusters = gridDim.x >> 1;
-  const int n_blocks = (g.c_out + CBN - 1) / CBN;
-  const int c_blocks = (g.c_in + BK - 1) / BK;
-  const int taps = g.kt * g.kh * g.kw;
-  const int k_iters = taps * c_blocks;
-  const long long m_tiles = static_cast<long long>(g.nb) * g.t_out * g.tiles_w * g.tiles_h;
-  const long long pairs = (m_tiles + 1) / 2;
-  const long long num_tiles = pairs * n_blocks;
-  // both CTAs' loads complete on the leader's barrier: 2 x (pixel patch + weight half)
-  const uint32_t stage_tx = 2u * static_cast<uint32_t>(g.bw * g.bh * BK * 2 + B_BYTES);
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_x);
-    tma_prefetch_desc(&tmap_w);
-    for (int s = 0; s < CV2_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], 2 * EPI_WARPS); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm(tmem_ptr, TMEM_COLS);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  // pair tile -> (n_blk fastest, then the pair of pixel tiles); this CTA's pixel tile
-  auto decode = [&](long long tile, int& n_blk, int& w0, int& h0, int& t, int& nb) -> bool {
-    n_blk = static_cast<int>(tile % n_blocks);
-    long long r = (tile / n_blocks) * 2 + rank;
-    const bool valid = r < m_tiles;
-    w0 = static_cast<int>(r % g.tiles_w) * g.bw; r /= g.tiles_w;
-    h0 = static_cast<int>(r % g.tiles_h) * g.bh; r /= g.tiles_h;
-    t = static_cast<int>(r % g.t_out);
-    nb = static_cast<int>(r / g.t_out);      // == g.nb for the dummy tile: out of bounds, zero fill
-    return valid;
-  };
-
-  if (warp == 0) {
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (long long tile = cluster_id; tile < num_tiles; tile += n_clusters) {
-        int n_blk, w0, h0, t, nb;
-        decode(tile, n_blk, w0, h0, t, nb);
-        for (int tap = 0; tap < taps; ++tap) {
-          const int dw = tap % g.kw, dh = (tap / g.kw) % g.kh, dt = tap / (g.kw * g.kh);
-          for (int cb = 0; cb < c_blocks; ++cb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            const uint32_t leader_full = mapa_u32(smem_u32(&full_bar[stage]), 0);
-            if (rank == 0) mbar_expect_tx(&full_bar[stage], stage_tx);
-            tma_load_5d_2sm(&tmap_x, leader_full, smem_a + stage * CV_A_BYTES, cb * BK, w0 + dw - g.kw / 2,
-                            h0 + dh - g.kh / 2, t + dt, nb, kEvictNormal);
-            tma_load_2d_2sm(&tmap_w, leader_full, smem_b + stage * B_BYTES, cb * BK,
-                            tap * g.c_out + n_blk * CBN + static_cast<int>(rank) * (CBN / 2), kEvictLast);
-            if (++stage == CV2_STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = umma_idesc(2 * BM, CBN, Cvt<T>::kUmmaFmt);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (long long tile = cluster_id; tile < num_tiles; tile += n_clusters, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * CBN;
-        for (int ki = 0; ki < k_iters; ++ki) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t da = umma_desc_sw128(smem_u32(smem_a + stage * CV_A_BYTES));
-          const uint64_t db = umma_desc_sw128(smem_u32(smem_b + stage * B_BYTES));
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k)
-            umma_f16_2sm(tmem_d, da + 2 * k, db + 2 * k, idesc, (ki | k) ? 1u : 0u);
-          umma_commit_2sm_mc(&empty_bar[stage]);
-          if (++stage == CV2_STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm_mc(&tfull_bar[as]);
-      }
-    }
-    __syncwarp();
-  } else {
-    const int quarter = warp & 3;
-    int it = 0;
-    for (long long tile = cluster_id; tile < num_tiles; tile += n_clusters, ++it) {
-      int n_blk, w0, h0, t, nb;
-      const bool valid = decode(tile, n_blk, w0, h0, t, nb);
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      if (valid) {
-        const uint32_t taddr = tmem_base + as * CBN + (static_cast<uint32_t>(quarter * 32) << 16);
-        TileGeom tg;
-        tg.bw = g.bw; tg.rows = g.bw * g.bh; tg.w_lim = g.w - w0; tg.h_lim = g.h - h0; tg.img_w = g.w;
-        tg.tile_cols = CBN;
-        const int m_base = ((nb * g.t_out + t) * g.h + h0) * g.w + w0;
-        drain_tile<T, EPI>(taddr, epi_stage + (warp - 2) * 256, m_base, quarter * 32, 0, n_blk * CBN, g.c_out, p,
-                           lane, (warp - 2) >> 2, tg);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(mapa_u32(smem_u32(&tempty_bar[as]), 0));
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Halo-row variant of the cta_group::2 kernel for kw = 3 and W >= 128.  The kernels above
-// re-read the shifted activation patch from L2 once per TAP: at C_out = 128 that is 94 B/clk/SM
-// of L2->SM operand traffic and the measured limiter (tensor pipe 47 %, DESIGN.md §3.4).  Here
-// an M tile is ONE image-row segment of 128 pixels; per (dt, dh, C_in block) the producer loads
-// the segment with a one-pixel halo on both sides ONCE (130 rows x 128 B, TMA zero fill = the
-// spatial padding) plus the three weight slices of dw = 0, 1, 2, and the MMA warp issues the three
-// taps against ROW-SHIFTED views of that one shared-memory tile: the UMMA descriptor simply
-// starts dw rows (dw x 128 B) into the tile.  Measured on B200 (tools/conv_halo_probe.py, r02):
-// the 128-byte swizzle phase follows the ABSOLUTE shared-memory address bits [7:9], exactly as
-// TMA wrote the tile, so a start address that is not aligned to the 1024-byte pattern needs NO
-// base-offset field (bits 49-51 = 0 is exact to 1e-6 against torch; = dw gives garbage).  A
-// traffic drops 3x (27 -> 9 loads per C_in block for 3x3x3).
+// Variants of one kernel (same pipeline, same epilogues):
+//   CL = 2    cluster of two CTAs on two pixel tiles that share the weight slice: each CTA loads
+//             its own shifted patch and HALF of the slice, multicast into both (protocol of the
+//             paired GEMM, gemm.cu); same accumulation order as CL = 1, so the same bits
+//   HALO      kw = 3 and rows of >= 128 pixels: an M tile is ONE image-row segment of 128
+//             pixels.  Per (dt, dh, C_in block) the producer loads the segment with a one-pixel
+//             halo on both sides ONCE (130 rows x 128 B; TMA zero fill = the spatial padding)
+//             plus the three weight slices of dw = 0, 1, 2, and the consumers issue the three
+//             taps against ROW-SHIFTED views of that tile (descriptor start dw rows in, base
+//             offset 0: the swizzle follows the absolute address).  A traffic drops 3x
+//             (27 -> 9 loads per C_in block for 3x3x3).
 constexpr int CVH_A_ROWS = 130;
 constexpr int CVH_A_BYTES = 17 * 1024;        // 130 rows x 128 B, rounded up to the swizzle pattern
 
-template <int CBN> struct CvhCfg {
-  static constexpr int kBBytes = (CBN / 2) * BK * 2;               // one tap's weight half
-  static constexpr int kStageBytes = CVH_A_BYTES + 3 * kBBytes;
-  static constexpr int kStages = 4;            // CBN <= 128: 4 x <= 41 KB
-  static constexpr int kSmemBytes = kStages * kStageBytes + EPI_STAGE_BYTES + 1024 + 256;
+template <int CBN, bool HALO>
+struct ConvCfg {
+  static constexpr int kTaps = HALO ? 3 : 1;                   // weight slices per stage
+  static constexpr int kABytes = HALO ? CVH_A_BYTES : CV_A_BYTES;
+  static constexpr int kBBytes = kTaps * CBN * BK * 2;
+  static constexpr int kStages = (kABytes + kBBytes) > 48 * 1024 ? 3 : CV_STAGES;
+  static constexpr int kSmemBytes = kStages * (kABytes + kBBytes) + EPI_STAGE_BYTES + 1024 + 256;
 };
 
-int g_conv_halo = -1;         // -1: env DWM_CONV_HALO (default 1); option "conv_halo"
-
-template <typename T, int EPI, int CBN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-    convh_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                         const ConvGeom g, EpiParams p) {
-  using Cfg = CvhCfg<CBN>;
-  constexpr int B_BYTES = Cfg::kBBytes;
-  constexpr int STAGES = Cfg::kStages;
+template <typename T, int EPI, int CBN, int CL, bool HALO>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+    conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+                      const ConvGeom g, EpiParams p) {
+  using Cfg = ConvCfg<CBN, HALO>;
+  constexpr int A_BYTES = Cfg::kABytes, B_BYTES = Cfg::kBBytes, STAGES = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float4* epi_stage = reinterpret_cast<float4*>(smem + STAGES * Cfg::kStageBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::kStageBytes + EPI_STAGE_BYTES);
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + STAGES * A_BYTES;
+  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * (A_BYTES + B_BYTES));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES) + EPI_STAGE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int cluster_id = blockIdx.x >> 1;
-  const int n_clusters = gridDim.x >> 1;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
+  const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
   const int n_blocks = (g.c_out + CBN - 1) / CBN;
   const int c_blocks = (g.c_in + BK - 1) / BK;
-  const int outer_taps = g.kt * g.kh;                       // (dt, dh); dw runs inside the stage
+  const int outer_taps = HALO ? g.kt * g.kh : g.kt * g.kh * g.kw;   // HALO: dw runs inside the stage
   const int k_iters = outer_taps * c_blocks;
-  const int w_tiles = (g.w + 127) / 128;
-  const long long m_tiles = static_cast<long long>(g.nb) * g.t_out * g.h * w_tiles;
-  const long long pairs = (m_tiles + 1) / 2;
-  const long long num_tiles = pairs * n_blocks;
-  const uint32_t stage_tx = 2u * static_cast<uint32_t>(CVH_A_ROWS * BK * 2 + 3 * B_BYTES);
+  const int w_tiles = HALO ? (g.w + 127) / 128 : g.tiles_w;
+  const long long m_tiles = static_cast<long long>(g.nb) * g.t_out * (HALO ? g.h * w_tiles : g.tiles_w * g.tiles_h);
+  const long long num_tiles = ((m_tiles + CL - 1) / CL) * n_blocks;
+  const long long first = static_cast<long long>(blockIdx.x) / CL, step = static_cast<long long>(gridDim.x) / CL;
+  const uint32_t stage_tx = HALO ? static_cast<uint32_t>(CVH_A_ROWS * BK * 2 + B_BYTES)
+                                 : static_cast<uint32_t>(g.bw * g.bh * BK * 2 + B_BYTES);
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_x);
     tma_prefetch_desc(&tmap_w);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], 2 * EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CL * EPI_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_2sm(tmem_ptr, TMEM_COLS);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
+  if constexpr (CL == 2) cluster_sync_all(); else __syncthreads();
 
-  // pair tile -> (n_blk fastest, then the pair of row segments); this CTA's segment
-  auto decode = [&](long long tile, int& n_blk, int& w0, int& h, int& t, int& nb) -> bool {
+  // tile -> (n_blk fastest, then the group of CL pixel tiles); this CTA's pixel tile: its
+  // (w0, h0) origin, frame and volume.  HALO tiles are row segments (bh = 1, bw = 128).  The
+  // dummy tile of an odd pair has nb == g.nb: out of bounds, zero fill, never stored.
+  auto decode = [&](long long tile, int& n_blk, int& w0, int& h0, int& t, int& nb) -> bool {
     n_blk = static_cast<int>(tile % n_blocks);
-    long long r = (tile / n_blocks) * 2 + rank;
+    long long r = (tile / n_blocks) * CL + rank;
     const bool valid = r < m_tiles;
-    w0 = static_cast<int>(r % w_tiles) * 128; r /= w_tiles;
-    h = static_cast<int>(r % g.h); r /= g.h;
+    if (HALO) {
+      w0 = static_cast<int>(r % w_tiles) * 128; r /= w_tiles;
+      h0 = static_cast<int>(r % g.h); r /= g.h;
+    } else {
+      w0 = static_cast<int>(r % g.tiles_w) * g.bw; r /= g.tiles_w;
+      h0 = static_cast<int>(r % g.tiles_h) * g.bh; r /= g.tiles_h;
+    }
     t = static_cast<int>(r % g.t_out);
-    nb = static_cast<int>(r / g.t_out);      // == g.nb for the dummy tile: out of bounds, zero fill
+    nb = static_cast<int>(r / g.t_out);
     return valid;
   };
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (wg == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (long long tile = cluster_id; tile < num_tiles; tile += n_clusters) {
-        int n_blk, w0, h, t, nb;
-        decode(tile, n_blk, w0, h, t, nb);
+      for (long long tile = first; tile < num_tiles; tile += step) {
+        int n_blk, w0, h0, t, nb;
+        decode(tile, n_blk, w0, h0, t, nb);
         for (int ot = 0; ot < outer_taps; ++ot) {
-          const int dh = ot % g.kh, dt = ot / g.kh;
+          const int kw_in = HALO ? 1 : g.kw;
+          const int dw = ot % kw_in, dh = (ot / kw_in) % g.kh, dt = ot / (kw_in * g.kh);
           for (int cb = 0; cb < c_blocks; ++cb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* st = smem + stage * Cfg::kStageBytes;
-            const uint32_t leader_full = mapa_u32(smem_u32(&full_bar[stage]), 0);
-            if (rank == 0) mbar_expect_tx(&full_bar[stage], stage_tx);
-            tma_load_5d_2sm(&tmap_x, leader_full, st, cb * BK, w0 - 1, h + dh - g.kh / 2, t + dt, nb, kEvictNormal);
+            mbar_expect_tx(&full_bar[stage], stage_tx);
+            uint8_t* sb = smem_b + stage * B_BYTES;
+            if constexpr (HALO) {
+              tma_load_5d(&tmap_x, &full_bar[stage], smem_a + stage * A_BYTES, cb * BK, w0 - 1,
+                          h0 + dh - g.kh / 2, t + dt, nb, kEvictNormal);
 #pragma unroll
-            for (int dw = 0; dw < 3; ++dw)
-              tma_load_2d_2sm(&tmap_w, leader_full, st + CVH_A_BYTES + dw * B_BYTES, cb * BK,
-                              (ot * 3 + dw) * g.c_out + n_blk * CBN + static_cast<int>(rank) * (CBN / 2), kEvictLast);
+              for (int d = 0; d < 3; ++d)
+                tma_load_2d(&tmap_w, &full_bar[stage], sb + d * CBN * BK * 2, cb * BK,
+                            (ot * 3 + d) * g.c_out + n_blk * CBN, kEvictLast);
+            } else {
+              tma_load_5d(&tmap_x, &full_bar[stage], smem_a + stage * A_BYTES, cb * BK,
+                          w0 + dw - g.kw / 2, h0 + dh - g.kh / 2, t + dt, nb, kEvictNormal);
+              if constexpr (CL == 2)
+                tma_load_2d_mc(&tmap_w, &full_bar[stage], sb + rank * (B_BYTES / 2), cb * BK,
+                               ot * g.c_out + n_blk * CBN + static_cast<int>(rank) * (CBN / 2), 0x3, kEvictLast);
+              else
+                tma_load_2d(&tmap_w, &full_bar[stage], sb, cb * BK, ot * g.c_out + n_blk * CBN, kEvictLast);
+            }
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = umma_idesc(2 * BM, CBN, Cvt<T>::kUmmaFmt);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (long long tile = cluster_id; tile < num_tiles; tile += n_clusters, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * CBN;
-        for (int ki = 0; ki < k_iters; ++ki) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t st = smem_u32(smem + stage * Cfg::kStageBytes);
-#pragma unroll
-          for (int dw = 0; dw < 3; ++dw) {
-            const uint64_t da = umma_desc_sw128(st + dw * 128u);       // row-shifted view
-            const uint64_t db = umma_desc_sw128(st + CVH_A_BYTES + dw * B_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k)
-              umma_f16_2sm(tmem_d, da + 2 * k, db + 2 * k, idesc, (ki | dw | k) ? 1u : 0u);
-          }
-          umma_commit_2sm_mc(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm_mc(&tfull_bar[as]);
-      }
-    }
-    __syncwarp();
   } else {
-    const int quarter = warp & 3;
-    int it = 0;
-    for (long long tile = cluster_id; tile < num_tiles; tile += n_clusters, ++it) {
-      int n_blk, w0, h, t, nb;
-      const bool valid = decode(tile, n_blk, w0, h, t, nb);
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      if (valid) {
-        const uint32_t taddr = tmem_base + as * CBN + (static_cast<uint32_t>(quarter * 32) << 16);
-        TileGeom tg;
-        tg.bw = 128; tg.rows = 128; tg.w_lim = g.w - w0; tg.h_lim = 1; tg.img_w = g.w;
-        tg.tile_cols = CBN;
-        const int m_base = ((nb * g.t_out + t) * g.h + h) * g.w + w0;
-        drain_tile<T, EPI>(taddr, epi_stage + (warp - 2) * 256, m_base, quarter * 32, 0, n_blk * CBN, g.c_out, p,
-                           lane, (warp - 2) >> 2, tg);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(mapa_u32(smem_u32(&tempty_bar[as]), 0));
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int cw = wg - 1;
+    const int wrow = cw * 64 + (warp & 3) * 16;
+    float* stg = epi_stage + (warp - 4) * 512;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (long long tile = first; tile < num_tiles; tile += step) {
+      int n_blk, w0, h0, t, nb;
+      const bool valid = decode(tile, n_blk, w0, h0, t, nb);
+      float acc[CBN / 2];
+      wg_mainloop<T, CBN, CL, Cfg::kTaps>(acc, smem_a, A_BYTES, cw * 64 * 128, smem_b, B_BYTES, full_bar, empty_bar,
+                                          STAGES, k_iters, stage, phase, lane, rank ^ 1u);
+      if (!valid) continue;
+      TileGeom tg;
+      tg.bw = HALO ? 128 : g.bw; tg.rows = HALO ? 128 : g.bw * g.bh;
+      tg.w_lim = g.w - w0; tg.h_lim = HALO ? 1 : g.h - h0; tg.img_w = g.w;
+      const int m_base = ((nb * g.t_out + t) * g.h + h0) * g.w + w0;
+      drain_tile<T, EPI, CBN>(acc, stg, m_base, wrow, 0, n_blk * CBN, g.c_out, p, lane, tg);
     }
   }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, TMEM_COLS);
-  }
+  if constexpr (CL == 2) cluster_sync_all();
 }
-
-int g_conv_2cta = -1;   // -1: env DWM_CONV_2CTA (default 1); dwm_b200_set_option("conv_2cta", 0 | 1)
 
 int make_tmap_nd(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                  const uint32_t* box, int elem_bytes);   // host.cu
+
+extern int g_conv_2cta, g_conv_halo;
 
 template <typename T, int EPI, int CBN>
 static int launch_conv(const dwm_conv_args* a, cudaStream_t stream) {
@@ -515,76 +206,58 @@ static int launch_conv(const dwm_conv_args* a, cudaStream_t stream) {
   p.n_peers = 0;
 
   const long long n_blocks = (g.c_out + CBN - 1) / CBN;
-  const long long tiles = static_cast<long long>(g.nb) * g.t_out * g.tiles_w * g.tiles_h * n_blocks;
+  const long long m_tiles = static_cast<long long>(g.nb) * g.t_out * g.tiles_w * g.tiles_h;
+  const long long seg_tiles = static_cast<long long>(g.nb) * g.t_out * g.h * ((g.w + 127) / 128);
   const int sms = sm_count();
   if (g_conv_2cta < 0) {
     const char* e = getenv("DWM_CONV_2CTA");
     g_conv_2cta = (e && e[0] == '0') ? 0 : 1;
   }
-  // cta_group::2 pairs once there are enough pixel tiles to fill the SM pairs (CBN >= 64: the
-  // W half of a pair must be a whole 8-row swizzle atom per CTA)
-  if constexpr (CBN >= 64) {
-    if (g_conv_halo < 0) {
-      const char* e = getenv("DWM_CONV_HALO");
-      g_conv_halo = (e && e[0] == '0') ? 0 : 1;
+  if (g_conv_halo < 0) {
+    const char* e = getenv("DWM_CONV_HALO");
+    g_conv_halo = (e && e[0] == '0') ? 0 : 1;
+  }
+  // shared-memory opt-in once per kernel instantiation (one flag per variant)
+  static bool attr_halo = false, attr_pair = false, attr_one = false;
+  auto go = [&](auto kern, bool& attr_set, int smem_bytes, int cl, long long mt, const CUtensorMap& x,
+                const CUtensorMap& w) -> int {
+    if (!attr_set) {
+      DWM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+      attr_set = true;
     }
-    // halo-row kernel: kw = 3, rows of at least 128 pixels, enough row segments for the pairs
-    const long long seg_tiles = static_cast<long long>(g.nb) * g.t_out * g.h * ((g.w + 127) / 128) * n_blocks;
-    // (C_out tiles of 256 columns are MMA-bound already — 94 % tensor pipe — and their three
-    // weight slices per stage would not fit)
-    if (CBN <= 128 && g_conv_2cta == 1 && g_conv_halo == 1 && a->kw == 3 && g.w >= 128 && seg_tiles >= 2 * sms) {
-      using Cfg = CvhCfg<(CBN <= 128 ? CBN : 128)>;
+    const long long tiles = ((mt + cl - 1) / cl) * n_blocks;
+    const long long slots = sms / cl;
+    const int grid = cl * static_cast<int>(tiles < slots ? tiles : slots);
+    if (cl == 1) kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(x, w, g, p);
+    else DWM_CHECK_CUDA(launch_cluster2(kern, grid, GEMM_THREADS, smem_bytes, stream, x, w, g, p));
+    DWM_CHECK_CUDA(cudaGetLastError());
+    return 0;
+  };
+  if constexpr (CBN <= 128) {
+    // halo-row kernel: kw = 3, rows of at least 128 pixels, enough row segments for the SMs
+    // (C_out tiles of 256 columns: three weight slices per stage would not fit)
+    if (g_conv_halo == 1 && a->kw == 3 && g.w >= 128 && seg_tiles * n_blocks >= sms) {
       CUtensorMap txh;
       const uint32_t boxh[5] = {BK, static_cast<uint32_t>(CVH_A_ROWS), 1, 1, 1};
       rc = make_tmap_nd(&txh, a->x, 5, dims, st, boxh, 2);
       if (rc) return rc;
-      rc = make_tmap_2d(&tw, a->weight, static_cast<uint64_t>(taps) * a->c_out, a->c_in, a->c_in, CBN / 2, BK, 2);
-      if (rc) return rc;
-      auto kernh = convh_tcgen05_kernel<T, EPI, (CBN <= 128 ? CBN : 128)>;
-      static bool attrh_set = false;
-      if (!attrh_set) {
-        DWM_CHECK_CUDA(cudaFuncSetAttribute(kernh, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-        attrh_set = true;
-      }
-      const long long ptiles = ((seg_tiles / n_blocks + 1) / 2) * n_blocks;
-      const int pairs = sms / 2;
-      const int clusters = static_cast<int>(ptiles < pairs ? ptiles : pairs);
-      kernh<<<2 * clusters, GEMM_THREADS, Cfg::kSmemBytes, stream>>>(txh, tw, g, p);
-      DWM_CHECK_CUDA(cudaGetLastError());
-      return 0;
-    }
-    if (g_conv_2cta == 1 && tiles >= 2 * sms) {
-      // weight box = half of the CBN rows
-      rc = make_tmap_2d(&tw, a->weight, static_cast<uint64_t>(taps) * a->c_out, a->c_in, a->c_in, CBN / 2, BK, 2);
-      if (rc) return rc;
-      auto kern2 = conv2_tcgen05_kernel<T, EPI, CBN>;
-      constexpr int smem2 = CV2_STAGES * (CV_A_BYTES + (CBN / 2) * BK * 2) + EPI_STAGE_BYTES + 1024 + 256;
-      static bool attr2_set = false;
-      if (!attr2_set) {
-        DWM_CHECK_CUDA(cudaFuncSetAttribute(kern2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2));
-        attr2_set = true;
-      }
-      const long long m_tiles = tiles / n_blocks;
-      const long long ptiles = ((m_tiles + 1) / 2) * n_blocks;
-      const int pairs = sms / 2;
-      const int clusters = static_cast<int>(ptiles < pairs ? ptiles : pairs);
-      kern2<<<2 * clusters, GEMM_THREADS, smem2, stream>>>(tx, tw, g, p);
-      DWM_CHECK_CUDA(cudaGetLastError());
-      return 0;
+      return go(conv_wgmma_kernel<T, EPI, CBN, 1, true>, attr_halo, ConvCfg<CBN, true>::kSmemBytes, 1, seg_tiles, txh, tw);
     }
   }
-  auto kern = conv_tcgen05_kernel<T, EPI, CBN>;
-  constexpr int smem_bytes = CV_STAGES * (CV_A_BYTES + CBN * BK * 2) + EPI_STAGE_BYTES + 1024 + 256;
-  static bool attr_set = false;
-  if (!attr_set) {
-    DWM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    attr_set = true;
+  if constexpr (CBN >= 64) {
+    // pairs once there are enough pixel tiles for both CTAs of every cluster (the weight half
+    // of a CTA must be whole 8-row swizzle atoms)
+    if (g_conv_2cta == 1 && m_tiles * n_blocks >= 2 * sms) {
+      rc = make_tmap_2d(&tw, a->weight, static_cast<uint64_t>(taps) * a->c_out, a->c_in, a->c_in, CBN / 2, BK, 2);
+      if (rc) return rc;
+      return go(conv_wgmma_kernel<T, EPI, CBN, 2, false>, attr_pair, ConvCfg<CBN, false>::kSmemBytes, 2, m_tiles, tx, tw);
+    }
   }
-  const int grid = static_cast<int>(tiles < sms ? tiles : sms);
-  kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(tx, tw, g, p);
-  DWM_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return go(conv_wgmma_kernel<T, EPI, CBN, 1, false>, attr_one, ConvCfg<CBN, false>::kSmemBytes, 1, m_tiles, tx, tw);
 }
+
+int g_conv_2cta = -1;   // -1: env DWM_CONV_2CTA (default 1); option "conv_2cta"
+int g_conv_halo = -1;   // -1: env DWM_CONV_HALO (default 1); option "conv_halo"
 
 template <typename T, int EPI>
 static int conv_pick_bn(const dwm_conv_args* a, cudaStream_t s) {

@@ -1,16 +1,15 @@
-// Persistent warp-specialised tcgen05 GEMM with fused epilogues (sm_100a).
+// Persistent warp-specialised wgmma GEMM with fused epilogues (sm_90a).
 //
-//   D[M,N] = A[M,K] · W[N,K]^T     A, W 16-bit (bf16/fp16), fp32 accumulation in TMEM
+//   D[M,N] = A[M,K] · W[N,K]^T     A, W 16-bit (bf16/fp16), fp32 accumulation in registers
 //
-// Roles (320 threads, one CTA per SM, persistent over output tiles):
-//   warp 0    TMA producer: 128x64 A tile + 256x64 W tile per k-block into a
-//             4-stage 128B-swizzled shared-memory ring (mbarrier tx-count completion)
-//   warp 1    MMA issuer: one elected thread issues tcgen05.mma 128x256x16, commits
-//             stage release and accumulator-ready to mbarriers; owns TMEM alloc
-//   warps 2-9 epilogue: tcgen05.ld the 128x256 fp32 accumulator (lane = row; two warps
-//             per TMEM lane quarter, interleaved over 32-column chunks), apply the fused
-//             epilogue and store; double-buffered TMEM (2 x 256 columns) so the
-//             epilogue of tile i overlaps the main loop of tile i+1
+// Roles (384 threads, one CTA per SM, persistent over 128 x NT output tiles):
+//   warpgroup 0    TMA producer (one elected thread): 128x64 A tile + NTx64 W tile per k-block
+//                  into a 4-stage 128B-swizzled shared-memory ring (mbarrier tx-count completion);
+//                  runs ahead into the next tile while the consumers drain the current one
+//   warpgroups 1-2 consumers: each issues wgmma m64nNTk16 for its 64 rows of the tile and
+//                  then applies the fused epilogue straight from its register fragment
+// NT = 256 (the widest wgmma; 128 accumulator registers per thread) unless a 128-wide tile
+// gives the last wave fewer idle SMs.
 //
 // Replaces the cuBLASLt GEMM + ~10 elementwise launches per sub-layer that the
 // reference runs (SURVEY.md §2.3 K5-K8).
@@ -23,198 +22,192 @@ namespace dwm {
 
 constexpr int STAGES = 4;
 constexpr int A_STAGE_BYTES = BM * BK * 2;
-constexpr int B_STAGE_BYTES = BN * BK * 2;
-constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr int GEMM_SMEM_BYTES =
-    STAGES * STAGE_BYTES + EPI_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 
-template <typename T, int EPI>
+template <int NT>
+struct GemmCfg {
+  static constexpr int kBStageBytes = NT * BK * 2;
+  static constexpr int kSmemBytes =
+      STAGES * (A_STAGE_BYTES + kBStageBytes) + EPI_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+};
+
+// CL = 2: a cluster of two CTAs computes two vertically adjacent output tiles that share one
+// W tile; each CTA loads its own A tile and HALF of the W tile, multicast into both CTAs, so
+// every CTA reads half as much weight data from L2.  A stage of a CTA is refilled only after
+// the consumers of BOTH CTAs have released it (the peer writes into it too).  An odd number
+// of M tiles gives the last pair a dummy tile: its A loads are out of bounds (zero fill) and
+// its rows are never stored.  Both variants accumulate in the same order: same bits.
+template <typename T, int EPI, int NT, int CL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-    gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                        const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
-                        EpiParams p) {
+    gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                      const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
+                      EpiParams p) {
+  constexpr int B_STAGE_BYTES = GemmCfg<NT>::kBStageBytes;
   extern __shared__ uint8_t smem_raw[];
-  // 128B-swizzled UMMA/TMA tiles need 1024-byte alignment.
+  // 128B-swizzled TMA / wgmma tiles need 1024-byte alignment.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  float4* epi_stage = reinterpret_cast<float4*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + EPI_STAGE_BYTES);
-  uint64_t* full_bar = bars;                 // [STAGES]  TMA -> MMA
-  uint64_t* empty_bar = bars + STAGES;       // [STAGES]  MMA -> TMA
-  uint64_t* tfull_bar = bars + 2 * STAGES;   // [2]       MMA -> epilogue
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2;  // [2]   epilogue -> MMA
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + EPI_STAGE_BYTES);
+  uint64_t* full_bar = bars;                 // [STAGES]  TMA -> consumers
+  uint64_t* empty_bar = bars + STAGES;       // [STAGES]  consumers (of both CTAs when CL = 2) -> TMA
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
 
   const int m_blocks = (M + BM - 1) / BM;
-  const int n_blocks = (N + BN - 1) / BN;
+  const int n_blocks = (N + NT - 1) / NT;
   const int k_blocks = (K + BK - 1) / BK;
-  const int num_tiles = m_blocks * n_blocks;
+  const int num_tiles = ((m_blocks + CL - 1) / CL) * n_blocks;   // CL vertically adjacent tiles each
+  const int first = static_cast<int>(blockIdx.x) / CL, step = static_cast<int>(gridDim.x) / CL;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], EPI_WARPS);
+      mbar_init(&empty_bar[s], CL * EPI_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
+  if constexpr (CL == 2) cluster_sync_all(); else __syncthreads();
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_blocks;
+      for (int tile = first; tile < num_tiles; tile += step) {
+        const int m_blk = (tile / n_blocks) * CL + static_cast<int>(rank);
         const int n_blk = tile % n_blocks;
         for (int kb = 0; kb < k_blocks; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+          mbar_expect_tx(&full_bar[stage], A_STAGE_BYTES + B_STAGE_BYTES);
           tma_load_2d(&tmap_a, &full_bar[stage], smem_a + stage * A_STAGE_BYTES, kb * BK,
                       m_blk * BM, kEvictNormal);
-          tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES, kb * BK,
-                      n_blk * BN, kEvictLast);
+          if constexpr (CL == 2) {
+            tma_load_2d_mc(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES + rank * (B_STAGE_BYTES / 2),
+                           kb * BK, n_blk * NT + static_cast<int>(rank) * (NT / 2), 0x3, kEvictLast);
+          } else {
+            tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES, kb * BK,
+                        n_blk * NT, kEvictLast);
+          }
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
           }
         }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc(BM, BN, Cvt<T>::kUmmaFmt);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t da = umma_desc_sw128(smem_u32(smem_a + stage * A_STAGE_BYTES));
-          const uint64_t db = umma_desc_sw128(smem_u32(smem_b + stage * B_STAGE_BYTES));
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            // advance 16 elements (32 B) along K inside the 128B swizzle atom
-            umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull_bar[as]);
       }
     }
     __syncwarp();
   } else {
-    // ===================== epilogue (warps 2..9) =====================
-    const int quarter = warp & 3;  // TMEM lane quarter this warp may access
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int m_blk = tile / n_blocks;
+    // ===================== consumers (warpgroups 1, 2) =====================
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int cw = wg - 1;                       // 64-row half of the tile
+    const int wrow = cw * 64 + (warp & 3) * 16;  // first tile row of this warp
+    float* stg = epi_stage + (warp - 4) * 512;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = first; tile < num_tiles; tile += step) {
+      const int m_blk = (tile / n_blocks) * CL + static_cast<int>(rank);
       const int n_blk = tile % n_blocks;
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      prefetch_resid_tile<EPI>(p, m_blk * BM + quarter * 32 + lane, M, n_blk * BN, N, (warp - 2) >> 2);
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + as * BN + (static_cast<uint32_t>(quarter * 32) << 16);
-      drain_tile<T, EPI>(taddr, epi_stage + (warp - 2) * 256, m_blk * BM, quarter * 32, M,
-                         n_blk * BN, N, p, lane, (warp - 2) >> 2);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[as]);
+      const int t = threadIdx.x & 127;
+      prefetch_resid_tile<EPI, NT>(p, m_blk * BM + cw * 64 + (t >> 1), M, n_blk * NT, N, t & 1);
+      float acc[NT / 2];
+      wg_mainloop<T, NT, CL>(acc, smem_a, A_STAGE_BYTES, cw * 64 * 128, smem_b, B_STAGE_BYTES, full_bar,
+                             empty_bar, STAGES, k_blocks, stage, phase, lane, rank ^ 1u);
+      drain_tile<T, EPI, NT>(acc, stg, m_blk * BM, wrow, M, n_blk * NT, N, p, lane);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
+  // a CTA of a pair must not exit while its peer may still multicast into it or arrive on it
+  if constexpr (CL == 2) cluster_sync_all();
 }
 
-template <typename T, int EPI>
+int g_resid_tma = 1;   // option "resid_tma": L2 prefetch of the RESID operands by the TMA unit
+
+template <typename T, int EPI, int NT, int CL>
 static int launch_gemm(const dwm_linear_args* a, cudaStream_t stream) {
   CUtensorMap ta, tb;
   int rc = make_tmap_2d(&ta, a->A, a->M, a->K, a->lda, BM, BK, 2);
   if (rc) return rc;
-  rc = make_tmap_2d(&tb, a->W, a->N, a->K, a->ldw, BN, BK, 2);
+  rc = make_tmap_2d(&tb, a->W, a->N, a->K, a->ldw, NT / CL, BK, 2);
   if (rc) return rc;
 
   EpiParams p;
   fill_epi_params(p, a);
+  p.resid_prefetch = g_resid_tma;
 
-  auto kern = gemm_tcgen05_kernel<T, EPI>;
+  constexpr int smem_bytes = GemmCfg<NT>::kSmemBytes;
+  auto kern = gemm_wgmma_kernel<T, EPI, NT, CL>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
-    DWM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        GEMM_SMEM_BYTES));
+    DWM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     attr_set = true;
   }
   const long long m_blocks = (a->M + BM - 1) / BM;
-  const long long n_blocks = (a->N + BN - 1) / BN;
-  const long long tiles = m_blocks * n_blocks;
-  const int sms = sm_count();
-  const int grid = static_cast<int>(tiles < sms ? tiles : sms);
-  kern<<<grid, GEMM_THREADS, GEMM_SMEM_BYTES, stream>>>(ta, tb, static_cast<int>(a->M),
-                                                        static_cast<int>(a->N),
-                                                        static_cast<int>(a->K), p);
+  const long long n_blocks = (a->N + NT - 1) / NT;
+  const long long tiles = ((m_blocks + CL - 1) / CL) * n_blocks;
+  const long long slots = sm_count() / CL;
+  const int grid = CL * static_cast<int>(tiles < slots ? tiles : slots);
+  const int Mi = static_cast<int>(a->M), Ni = static_cast<int>(a->N), Ki = static_cast<int>(a->K);
+  if constexpr (CL == 1) {
+    kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(ta, tb, Mi, Ni, Ki, p);
+  } else {
+    DWM_CHECK_CUDA(launch_cluster2(kern, grid, GEMM_THREADS, smem_bytes, stream,
+                                   ta, tb, Mi, Ni, Ki, p));
+  }
   DWM_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
-template <typename T>
+int g_gemm_bn = 0;   // 0: tile width by wave efficiency; 128 / 256 force it (option "gemm_bn")
+int g_gemm_2cta = -1;   // -1: from env DWM_GEMM_2CTA (default 1), 0 / 1: forced (option "gemm_2cta")
+
+// Time of a persistent launch ~ waves x tile width: the 128-wide tile wins when the 256-wide
+// tiles leave a last wave that is mostly idle SMs.
+static int pick_tile_n(const dwm_linear_args* a, int cl) {
+  if (a->epilogue == DWM_EPI_GEGLU) return 256;
+  if (g_gemm_bn == 128 || g_gemm_bn == 256) return g_gemm_bn;
+  const long long slots = sm_count() / cl;
+  const long long m_groups = ((a->M + BM - 1) / BM + cl - 1) / cl;
+  const long long t256 = m_groups * ((a->N + 255) / 256), t128 = m_groups * ((a->N + 127) / 128);
+  const long long cost256 = ((t256 + slots - 1) / slots) * 256, cost128 = ((t128 + slots - 1) / slots) * 128;
+  return cost128 < cost256 ? 128 : 256;
+}
+
+template <typename T, int EPI, int CL>
+static int launch_pick_n(const dwm_linear_args* a, cudaStream_t s) {
+  if (pick_tile_n(a, CL) == 128) return launch_gemm<T, EPI, 128, CL>(a, s);
+  return launch_gemm<T, EPI, 256, CL>(a, s);
+}
+
+template <typename T, int CL>
 static int dispatch_epi(const dwm_linear_args* a, cudaStream_t s) {
   switch (a->epilogue) {
-    case DWM_EPI_STORE: return launch_gemm<T, DWM_EPI_STORE>(a, s);
-    case DWM_EPI_GEGLU: return launch_gemm<T, DWM_EPI_GEGLU>(a, s);
-    case DWM_EPI_QKNORM: return launch_gemm<T, DWM_EPI_QKNORM>(a, s);
-    case DWM_EPI_RESID: return launch_gemm<T, DWM_EPI_RESID>(a, s);
-    case DWM_EPI_F32: return launch_gemm<T, DWM_EPI_F32>(a, s);
+    case DWM_EPI_STORE: return launch_pick_n<T, DWM_EPI_STORE, CL>(a, s);
+    case DWM_EPI_GEGLU: return launch_gemm<T, DWM_EPI_GEGLU, 256, CL>(a, s);
+    case DWM_EPI_QKNORM: return launch_pick_n<T, DWM_EPI_QKNORM, CL>(a, s);
+    case DWM_EPI_RESID: return launch_pick_n<T, DWM_EPI_RESID, CL>(a, s);
+    case DWM_EPI_F32: return launch_pick_n<T, DWM_EPI_F32, CL>(a, s);
     default: set_last_error("dwm_b200_linear: unknown epilogue %d", a->epilogue); return -1;
   }
 }
 
-int gemm2_launch(const dwm_linear_args* a, cudaStream_t s);   // gemm2.cu
-int g_gemm_2cta = -1;   // -1: from env DWM_GEMM_2CTA (default 1), 0 / 1: forced
-
 }  // namespace dwm
 
-namespace dwm { int g_attn_tc = -1; extern int g_ln_staged; extern int g_resid_tma; extern int g_gemm_bn; extern int g_conv_2cta; extern int g_conv_halo; }
+namespace dwm { int g_attn_tc = -1; extern int g_ln_staged; extern int g_conv_2cta; extern int g_conv_halo; }
 
 extern "C" int dwm_b200_set_option(const char* name, int value) {
   using namespace dwm;
   DWM_REQUIRE(name != nullptr, "dwm_b200_set_option: null name");
-  if (strcmp(name, "gemm_2cta") == 0) { g_gemm_2cta = value; return 0; }
   if (strcmp(name, "attn_tc") == 0) { g_attn_tc = value; return 0; }
   if (strcmp(name, "ln_staged") == 0) { g_ln_staged = value; return 0; }
-  if (strcmp(name, "resid_tma") == 0) { g_resid_tma = value; return 0; }
   if (strcmp(name, "gemm_bn") == 0) { g_gemm_bn = value; return 0; }
+  if (strcmp(name, "gemm_2cta") == 0) { g_gemm_2cta = value; return 0; }
+  if (strcmp(name, "resid_tma") == 0) { g_resid_tma = value; return 0; }
   if (strcmp(name, "conv_2cta") == 0) { g_conv_2cta = value; return 0; }
   if (strcmp(name, "conv_halo") == 0) { g_conv_halo = value; return 0; }
   set_last_error("dwm_b200_set_option: unknown option %s", name);
@@ -256,10 +249,10 @@ extern "C" int dwm_b200_linear(const dwm_linear_args* a, dwm_stream_t stream) {
     const char* e = getenv("DWM_GEMM_2CTA");
     g_gemm_2cta = (e && e[0] == '0') ? 0 : 1;
   }
-  // 2-CTA clusters pay off once there are enough 256-row tiles to fill the 74 SM pairs
-  if (g_gemm_2cta == 1 && a->M >= 512) return gemm2_launch(a, s);
-  if (a->dtype == DWM_BF16) return dispatch_epi<__nv_bfloat16>(a, s);
-  if (a->dtype == DWM_F16) return dispatch_epi<__half>(a, s);
+  // pairs pay off once there are enough 128-row tiles to give both CTAs of a cluster work
+  const bool pair = g_gemm_2cta == 1 && a->M >= 512;
+  if (a->dtype == DWM_BF16) return pair ? dispatch_epi<__nv_bfloat16, 2>(a, s) : dispatch_epi<__nv_bfloat16, 1>(a, s);
+  if (a->dtype == DWM_F16) return pair ? dispatch_epi<__half, 2>(a, s) : dispatch_epi<__half, 1>(a, s);
   set_last_error("dwm_b200_linear: dtype must be DWM_BF16 or DWM_F16, got %d", a->dtype);
   return -1;
 }

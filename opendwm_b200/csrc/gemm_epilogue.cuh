@@ -1,18 +1,22 @@
-// Fused-epilogue machinery shared by the 1-CTA and 2-CTA tcgen05 GEMM kernels.
+// Fused-epilogue machinery and the warpgroup main loop shared by the wgmma GEMM and
+// convolution kernels (sm_90a).
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "../../include/dwm_b200.h"
 
 namespace dwm {
 
-constexpr int BM = 128;   // accumulator rows per CTA (TMEM lanes)
-constexpr int BN = 256;
-constexpr int BK = 64;
-constexpr int UMMA_K = 16;
-constexpr int EPI_WARPS = 8;  // two warps per TMEM lane quarter, interleaved over column chunks
-constexpr int GEMM_THREADS = 64 + EPI_WARPS * 32;
-constexpr int TMEM_COLS = 512;
-constexpr int EPI_STAGE_BYTES = EPI_WARPS * 32 * 32 * 4;  // per epilogue warp: 32x32 fp32
+constexpr int BM = 128;   // accumulator rows per CTA: two consumer warpgroups x 64 rows
+constexpr int BK = 64;    // one 128-byte swizzle atom of 16-bit K per stage
+constexpr int WG_K = 16;
+constexpr int CONSUMER_WGS = 2;
+constexpr int GEMM_THREADS = 128 * (1 + CONSUMER_WGS);   // warpgroup 0: TMA producer
+constexpr int EPI_WARPS = 4 * CONSUMER_WGS;
+constexpr int EPI_STAGE_BYTES = EPI_WARPS * 16 * 32 * 4;  // per consumer warp: 16x32 fp32
+// register split (65536 per SM, one CTA): producer warpgroup 40, consumers 232 each
+constexpr int PRODUCER_REGS = 40;
+constexpr int CONSUMER_REGS = 232;
 
 struct EpiParams {
   void* out;
@@ -35,6 +39,7 @@ struct EpiParams {
   long long rows_per_batch;
   void* peer_out[8];
   int n_peers;
+  int resid_prefetch;   // RESID: L2 prefetch of the tile's residual / blend rows by the TMA unit
 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -64,21 +69,35 @@ __device__ __forceinline__ void st_global_v4(void* p, uint32_t a, uint32_t b, ui
                : "memory");
 }
 
-// ---- tile drain (4 epilogue warps) ----------------------------------------------
-// Each warp owns 32 accumulator rows (TMEM lane quarter).  tcgen05.ld hands every
-// thread one ROW, which would make global accesses 32-way scattered.  So each
-// 32x32 fp32 chunk is transposed through a 4 KB XOR-swizzled shared-memory
-// staging buffer: phase 1 (thread = row) applies the row-local math and dumps,
-// phase 2 (8 lanes per row, float4 per lane, 4 rows per instruction) does the
-// coalesced global traffic (incl. the fp32 residual read-modify-write).
+// ---- tile drain (consumer warps) -----------------------------------------------
+// Each consumer warp owns 16 accumulator rows of its warpgroup's 64 (wgmma fragment: lane l
+// holds rows l/4 and l/4 + 8, two adjacent columns per n8 block).  Per 32-column chunk the
+// warp applies the column-local math on the fragment, then transposes the 16x32 fp32 chunk
+// through a 2 KB XOR-swizzled shared-memory buffer (phase 1) so that the global traffic,
+// including the fp32 residual read-modify-write, is coalesced: 8 lanes per row, a float4
+// per lane, 4 rows per instruction (phase 2).
 
-__device__ __forceinline__ void stage_dump(float4* stg, int lane, const float (&v)[32]) {
-  __syncwarp();  // phase-2 readers of the previous chunk are done
+// chunk c of the fragment: v[4jj + e] = acc[4(4c + jj) + e]
+template <int NA>
+__device__ __forceinline__ void frag_chunk(const float (&acc)[NA], int c, float (&v)[16]) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j)
-    stg[lane * 8 + (j ^ (lane & 7))] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+  for (int i = 0; i < 16; ++i) v[i] = acc[16 * c + i];
+}
+
+__device__ __forceinline__ void stage_dump(float* stg, int lane, const float (&v)[16]) {
+  __syncwarp();  // phase-2 readers of the previous chunk are done
+  const int r0 = lane >> 2, q0 = (lane & 3) >> 1, h = (lane & 1) * 2;
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int q = (2 * jj + q0) ^ r0;       // float4 slot, swizzled by row (r0 + 8 has the same r & 7)
+    *reinterpret_cast<float2*>(stg + r0 * 32 + q * 4 + h) = make_float2(v[4 * jj], v[4 * jj + 1]);
+    *reinterpret_cast<float2*>(stg + (r0 + 8) * 32 + q * 4 + h) = make_float2(v[4 * jj + 2], v[4 * jj + 3]);
+  }
   __syncwarp();
 }
+
+// column of fragment value v[4jj + e] inside its 32-column chunk
+__device__ __forceinline__ int frag_col(int lane, int jj, int e) { return 8 * jj + 2 * (lane & 3) + (e & 1); }
 
 // Row mapping of an accumulator tile.  Linear (GEMM): tile row r is global row m_base + r,
 // valid while < M.  Pixel tile (implicit-GEMM convolution): the 128 accumulator rows are a
@@ -90,25 +109,25 @@ struct TileGeom {
   int w_lim;   // img_w - w0
   int h_lim;   // img_h - h0
   int img_w;
-  int tile_cols;   // accumulator columns of this tile (0 => BN)
 };
 
-template <typename T, int EPI>
-__device__ __forceinline__ void drain_tile(uint32_t taddr, float4* stg, int m_base, int row0, int M,
+// acc: the NT-column fragment of this warp's warpgroup; row0: tile row of the warp's first row
+template <typename T, int EPI, int NT>
+__device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* stg, int m_base, int row0, int M,
                                            int n_tile0, int N, const EpiParams& p, int lane,
-                                           int half, const TileGeom geom = TileGeom{0, 0, 0, 0, 0, 0}) {
+                                           const TileGeom geom = TileGeom{0, 0, 0, 0, 0}) {
   constexpr bool kOut16 = (EPI == DWM_EPI_STORE || EPI == DWM_EPI_GEGLU || EPI == DWM_EPI_QKNORM);
   const int rs = lane >> 3;  // phase-2: row within a group of 4
   const int c4 = lane & 7;   // phase-2: float4 column within the 32-col chunk
 
-  // phase-2 per-row metadata for the 8 rows this lane stores (it*4 + rs)
-  int orow[8];
-  int rrow[8];
-  int item[8];
-  float alpha[8];
+  // phase-2 per-row metadata for the 4 rows this lane stores (it*4 + rs)
+  int orow[4];
+  int rrow[4];
+  int item[4];
+  float alpha[4];
   const int rpi = static_cast<int>(p.rows_per_item);
 #pragma unroll
-  for (int it = 0; it < 8; ++it) {
+  for (int it = 0; it < 4; ++it) {
     int m;
     bool valid;
     if (geom.bw > 0) {
@@ -138,12 +157,12 @@ __device__ __forceinline__ void drain_tile(uint32_t taddr, float4* stg, int m_ba
     }
   }
 
+  auto stg4 = [&](int r) { return *reinterpret_cast<const float4*>(stg + r * 32 + ((c4 ^ (r & 7)) << 2)); };
   // phase 2 for 16-bit outputs: `ocol` = first output column of the staged chunk
   auto flush16 = [&](int ocol) {
 #pragma unroll
-    for (int it = 0; it < 8; ++it) {
-      const int r = it * 4 + rs;
-      const float4 v = stg[r * 8 + (c4 ^ (r & 7))];
+    for (int it = 0; it < 4; ++it) {
+      const float4 v = stg4(it * 4 + rs);
       if (orow[it] >= 0) {
         T* dst = reinterpret_cast<T*>(p.out) + static_cast<long long>(orow[it]) * p.ldo + ocol + c4 * 4;
         uint2 pk;
@@ -159,14 +178,14 @@ __device__ __forceinline__ void drain_tile(uint32_t taddr, float4* stg, int m_ba
   };
   // phase 2 for fp32 outputs (optionally gated / residual / blended).  The residual
   // (and blend) operands are prefetched into registers at the top of each chunk so
-  // their HBM latency overlaps the TMEM load + transpose; in-place update is safe
-  // because each lane reads exactly the elements it later writes.
-  float4 rq[8], bq[8];
+  // their HBM latency overlaps the transpose; in-place update is safe because each
+  // lane reads exactly the elements it later writes.
+  float4 rq[4], bq[4];
   auto prefetch32 = [&](int ocol) {
     if constexpr (EPI == DWM_EPI_RESID) {
       const int col = ocol + c4 * 4;
 #pragma unroll
-      for (int it = 0; it < 8; ++it) {
+      for (int it = 0; it < 4; ++it) {
         rq[it] = make_float4(0.f, 0.f, 0.f, 0.f);
         bq[it] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (orow[it] >= 0) {
@@ -181,9 +200,8 @@ __device__ __forceinline__ void drain_tile(uint32_t taddr, float4* stg, int m_ba
     float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
     if (EPI == DWM_EPI_RESID && p.bias) b = __ldg(reinterpret_cast<const float4*>(p.bias + col));
 #pragma unroll
-    for (int it = 0; it < 8; ++it) {
-      const int r = it * 4 + rs;
-      float4 v = stg[r * 8 + (c4 ^ (r & 7))];
+    for (int it = 0; it < 4; ++it) {
+      float4 v = stg4(it * 4 + rs);
       if (orow[it] >= 0) {
         if (EPI == DWM_EPI_RESID) {
           float4 g = make_float4(1.f, 1.f, 1.f, 1.f);
@@ -203,102 +221,101 @@ __device__ __forceinline__ void drain_tile(uint32_t taddr, float4* stg, int m_ba
   };
 
   if constexpr (EPI == DWM_EPI_STORE || EPI == DWM_EPI_F32 || EPI == DWM_EPI_RESID) {
-#pragma unroll 1
-    const int ncols = geom.tile_cols > 0 ? geom.tile_cols : BN;
-    for (int c = half; c * 32 < ncols; c += 2) {
+    // fully unrolled: the fragment is indexed with compile-time offsets only
+#pragma unroll
+    for (int c = 0; c < NT / 32; ++c) {
       const int n0 = n_tile0 + c * 32;
       if (n0 >= N) break;
       prefetch32(n0);
-      uint32_t r[32];
-      tmem_ld32(taddr + c * 32, r);
-      tmem_ld_wait();
-      float v[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
+      float v[16];
+      frag_chunk(acc, c, v);
       if (EPI != DWM_EPI_RESID) {
         if (p.bias) {
-          const float4* b4 = reinterpret_cast<const float4*>(p.bias + n0);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 b = __ldg(b4 + j);
-            v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
+          for (int jj = 0; jj < 4; ++jj) {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + frag_col(lane, jj, 0)));
+            v[4 * jj] += b.x; v[4 * jj + 1] += b.y; v[4 * jj + 2] += b.x; v[4 * jj + 3] += b.y;
           }
         }
         // activation selected once per chunk (warp-uniform), loops fully unrolled
         if (p.act == DWM_ACT_GELU_TANH) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_tanh(v[j]);
+          for (int j = 0; j < 16; ++j) v[j] = gelu_tanh(v[j]);
         } else if (p.act == DWM_ACT_SILU) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = silu(v[j]);
+          for (int j = 0; j < 16; ++j) v[j] = silu(v[j]);
         } else if (p.act == DWM_ACT_GELU_ERF) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
+          for (int j = 0; j < 16; ++j) v[j] = gelu_erf(v[j]);
         } else if (p.act == DWM_ACT_RELU) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
         }
       }
       stage_dump(stg, lane, v);
       if constexpr (EPI == DWM_EPI_STORE) flush16(n0); else flush32(n0);
     }
   } else if constexpr (EPI == DWM_EPI_GEGLU) {
+    static_assert(NT == 256, "GEGLU packs value / gate halves per 256-column tile");
     // tile columns [0,128) hold the value half, [128,256) the gate half of output
     // columns [n_tile0/2, n_tile0/2 + 128).
-#pragma unroll 1
-    for (int c = half; c < 4; c += 2) {
-      uint32_t rv[32], rg[32];
-      tmem_ld32(taddr + c * 32, rv);
-      tmem_ld32(taddr + 128 + c * 32, rg);
-      tmem_ld_wait();
-      const float* bv = p.bias ? p.bias + n_tile0 + c * 32 : nullptr;
-      float v[32];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        float a = __uint_as_float(rv[j]);
-        float g = __uint_as_float(rg[j]);
+    for (int c = 0; c < 4; ++c) {
+      float a[16], g[16], v[16];
+      frag_chunk(acc, c, a);
+      frag_chunk(acc, c + 4, g);
+      const float* bv = p.bias ? p.bias + n_tile0 + c * 32 : nullptr;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        float x = a[j], y = g[j];
         if (bv) {
-          a += __ldg(bv + j);
-          g += __ldg(bv + 128 + j);
+          const int col = frag_col(lane, j >> 2, j);
+          x += __ldg(bv + col);
+          y += __ldg(bv + 128 + col);
         }
-        v[j] = a * gelu_erf(g);
+        v[j] = x * gelu_erf(y);
       }
       stage_dump(stg, lane, v);
       flush16(n_tile0 / 2 + c * 32);
     }
   } else {  // DWM_EPI_QKNORM: 64-column heads
-#pragma unroll 1
-    for (int g = half; g < BN / 64; g += 2) {
+#pragma unroll
+    for (int g = 0; g < NT / 64; ++g) {
       const int n0 = n_tile0 + g * 64;
       if (n0 >= N) break;
-      uint32_t r0[32], r1[32];
-      tmem_ld32(taddr + g * 64, r0);
-      tmem_ld32(taddr + g * 64 + 32, r1);
-      tmem_ld_wait();
-      float v0[32], v1[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        v0[j] = __uint_as_float(r0[j]);
-        v1[j] = __uint_as_float(r1[j]);
-      }
+      float v0[16], v1[16];
+      frag_chunk(acc, 2 * g, v0);
+      frag_chunk(acc, 2 * g + 1, v1);
       if (p.bias) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          v0[j] += __ldg(p.bias + n0 + j);
-          v1[j] += __ldg(p.bias + n0 + 32 + j);
+        for (int j = 0; j < 16; ++j) {
+          const int col = frag_col(lane, j >> 2, j);
+          v0[j] += __ldg(p.bias + n0 + col);
+          v1[j] += __ldg(p.bias + n0 + 32 + col);
         }
       }
       const int region = n0 / static_cast<int>(p.qk_region);
       if (region < p.norm_regions) {
         const float* w = region == 0 ? p.qw : p.kw;
-        float ss = 0.f;
+        // a row's 64 values sit in the 4 lanes of a quad: e < 2 row l/4, e >= 2 row l/4 + 8
+        float ss_lo = 0.f, ss_hi = 0.f;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) ss += v0[j] * v0[j] + v1[j] * v1[j];
-        const float inv = rsqrtf(ss * (1.0f / 64.0f) + p.eps);
+        for (int j = 0; j < 16; ++j) {
+          if ((j & 3) < 2) ss_lo += v0[j] * v0[j] + v1[j] * v1[j];
+          else ss_hi += v0[j] * v0[j] + v1[j] * v1[j];
+        }
+        ss_lo += __shfl_xor_sync(0xffffffffu, ss_lo, 1);
+        ss_lo += __shfl_xor_sync(0xffffffffu, ss_lo, 2);
+        ss_hi += __shfl_xor_sync(0xffffffffu, ss_hi, 1);
+        ss_hi += __shfl_xor_sync(0xffffffffu, ss_hi, 2);
+        const float inv_lo = rsqrtf(ss_lo * (1.0f / 64.0f) + p.eps);
+        const float inv_hi = rsqrtf(ss_hi * (1.0f / 64.0f) + p.eps);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          v0[j] = v0[j] * inv * __ldg(w + j);
-          v1[j] = v1[j] * inv * __ldg(w + 32 + j);
+        for (int j = 0; j < 16; ++j) {
+          const int col = frag_col(lane, j >> 2, j);
+          const float inv = (j & 3) < 2 ? inv_lo : inv_hi;
+          v0[j] = v0[j] * inv * __ldg(w + col);
+          v1[j] = v1[j] * inv * __ldg(w + 32 + col);
         }
       }
       stage_dump(stg, lane, v0);
@@ -309,15 +326,56 @@ __device__ __forceinline__ void drain_tile(uint32_t taddr, float4* stg, int m_ba
   }
 }
 
+// One output tile of one consumer warpgroup: acc[64 x NT] = sum over k_iters stages and TAPS
+// taps of A[64 rows at a_row_off (+ t rows for tap t)] . B[NT rows of tap t]^T.  TAPS = 3 is
+// the halo-row convolution: the three dw taps read row-shifted views of one A tile.  Every stage
+// is released (one arrive per consumer warp, on this CTA's barrier and, in a cluster of two
+// that shares the B tile by multicast, on the peer's) as soon as the wgmma that read it has
+// completed; one wgmma group stays in flight.
+template <typename T, int NT, int CL = 1, int TAPS = 1>
+__device__ __forceinline__ void wg_mainloop(float (&acc)[NT / 2], const uint8_t* smem_a, int a_stage_bytes,
+                                            int a_row_off_bytes, const uint8_t* smem_b, int b_stage_bytes,
+                                            uint64_t* full_bar, uint64_t* empty_bar, int stages, int k_iters,
+                                            int& stage, uint32_t& phase, int lane, uint32_t peer = 0) {
+#pragma unroll
+  for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+  fence_operands(acc);
+  auto release = [&](int s) {
+    mbar_arrive(&empty_bar[s]);
+    if constexpr (CL == 2) mbar_arrive_remote(mapa_u32(smem_u32(&empty_bar[s]), peer));
+  };
+  int prev = -1;
+  for (int ki = 0; ki < k_iters; ++ki) {
+    mbar_wait(&full_bar[stage], phase);
+    wgmma_fence();
+#pragma unroll
+    for (int t = 0; t < TAPS; ++t) {
+      const uint64_t da = gmma_desc_sw128(smem_u32(smem_a + stage * a_stage_bytes + a_row_off_bytes + t * 128));
+      const uint64_t db = gmma_desc_sw128(smem_u32(smem_b + stage * b_stage_bytes + t * NT * BK * 2));
+#pragma unroll
+      for (int k = 0; k < BK / WG_K; ++k) Wgmma<NT, T>::ss(acc, da + 2 * k, db + 2 * k, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && lane == 0) release(prev);
+    prev = stage;
+    if (++stage == stages) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  fence_operands(acc);
+  if (prev >= 0 && lane == 0) release(prev);
+}
 
-// RESID epilogues read-modify-write a 128 KB fp32 tile whose HBM latency the 8 epilogue
+// RESID epilogues read-modify-write an fp32 tile of up to 128 KB whose HBM latency the 8 consumer
 // warps cannot cover with register prefetch alone.  While the MMAs of the tile are still
 // running, each epilogue thread asks the L2 to fetch its row segment (512 B) of the
 // residual (and blend) operand, so the later loads hit L2.
-template <int EPI>
+template <int EPI, int NT>
 __device__ __forceinline__ void prefetch_resid_tile(const EpiParams& p, int m, int M, int n_tile0,
-                                                    int N, int half, int half_cols = BN / 2) {
+                                                    int N, int half) {
+  constexpr int half_cols = NT / 2;
   if constexpr (EPI == DWM_EPI_RESID) {
+    if (!p.resid_prefetch) return;
     const int n0 = n_tile0 + half * half_cols;
     if (m < M && n0 < N) {
       const int cols = (N - n0) < half_cols ? (N - n0) : half_cols;
@@ -335,6 +393,25 @@ __device__ __forceinline__ void prefetch_resid_tile(const EpiParams& p, int m, i
       }
     }
   }
+}
+
+// host side: launches a kernel in clusters of two CTAs along x (grid must be even)
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_cluster2(void (*kern)(KArgs...), int grid, int threads, int smem, cudaStream_t s,
+                                   Args... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 
 // host side: fills EpiParams from the C-ABI struct
@@ -361,6 +438,7 @@ inline void fill_epi_params(EpiParams& p, const dwm_linear_args* a) {
   p.alpha = a->alpha;
   p.rows_per_batch = a->rows_per_batch;
   p.n_peers = a->n_peer_out;
+  p.resid_prefetch = 1;
   for (int i = 0; i < 8; ++i) p.peer_out[i] = i < a->n_peer_out ? a->peer_out[i] : nullptr;
 }
 

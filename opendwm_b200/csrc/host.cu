@@ -143,13 +143,13 @@ int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
 
 }  // namespace dwm
 
-extern "C" const char* dwm_b200_version(void) { return "dwm_b200 0.1 (sm_100a)"; }
+extern "C" const char* dwm_b200_version(void) { return "dwm_b200 0.1 (sm_90a)"; }
 extern "C" const char* dwm_b200_last_error(void) { return dwm::g_last_error; }

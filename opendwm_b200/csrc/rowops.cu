@@ -1,4 +1,4 @@
-// Memory-bound row / elementwise kernels of the CTSD step (sm_100a): LayerNorm with
+// Memory-bound row / elementwise kernels of the CTSD step (sm_90a): LayerNorm with
 // AdaLN modulation (emits the 16-bit GEMM operand), activation casts, sinusoidal
 // embeddings, patchify, and the fused CFG + un-patchify + per-frame Euler update.
 // All are single-pass over HBM with 128-bit accesses.

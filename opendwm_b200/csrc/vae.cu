@@ -143,8 +143,8 @@ struct SnParams {
 // position (t, h, w) advances by a constant number of pixels per iteration and is tracked with
 // carries instead of 64-bit divisions, the latent-grid coordinates are shifts when the sizes
 // are powers of two apart (always in the VAEs) and the frame map is a 64-entry shared table.
-// The r01 kernel spent ~10 integer divisions per float4 and ran at 18 % of DRAM peak
-// (profiles/r01_ncu_kernels_summary.txt); this one is a plain stream.
+// A version that spent ~10 integer divisions per float4 was far from DRAM-bound; this one is
+// a plain stream.
 template <typename T>
 __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, const int chunk) {
   // blockDim.x is a multiple of C/4 whenever C/4 <= 1024 (host side), `chunk` = blockDim.x * 16

@@ -5,8 +5,8 @@ blocks of diffusers.models.adapter (AdapterBlock / AdapterResnetBlock).
 The adapter does not depend on the latents or the timestep, yet the reference
 re-runs it inside every denoising forward (crossview_temporal_dit.py:459-462).  Here
 it is evaluated ONCE per condition set by the model's condition cache and its
-residuals are kept in token layout.  Its 1x1 convolutions run on the tcgen05 GEMM,
-its 3x3 convolutions on the im2col-free tcgen05 convolution (`dwm_b200_conv`, taps
+residuals are kept in token layout.  Its 1x1 convolutions run on the wgmma GEMM,
+its 3x3 convolutions on the im2col-free wgmma convolution (`dwm_b200_conv`, taps
 iterated inside the MMA loop over the channels-last feature map); no cuDNN kernel is
 involved.
 """

@@ -1,4 +1,4 @@
-"""2-D `AutoencoderKL` — decode path, B200-native (SURVEY.md §8(f)1).
+"""2-D `AutoencoderKL` — decode path, H100-native (SURVEY.md §8(f)1).
 
 Mirror of the part of diffusers==0.31.0 `AutoencoderKL` the reference uses at every
 emitted frame of the SD-2.1 / SD-3.5 image-VAE configs
@@ -8,12 +8,12 @@ constructor / config keys, `from_pretrained(path, subfolder="vae")`, state_dict 
 (`decoder.*`, `post_quant_conv.*`; encoder / quant_conv keys are ignored: encode is not on
 the path).
 
-Execution: activations are channels-last; every 3x3 convolution is the im2col-free tcgen05
+Execution: activations are channels-last; every 3x3 convolution is the im2col-free wgmma
 kernel (`dwm_b200_conv`, taps iterated inside the MMA loop, zero padding = TMA OOB fill)
 with the residual add as its epilogue; GroupNorm + SiLU is one statistics pass plus one
 fused apply pass that emits the next convolution's 16-bit input; nearest x2 upsampling
 writes the upsampler convolution's 16-bit input directly; the 1x1 shortcuts and the
-mid-block attention projections run on the tcgen05 GEMM.  The single-head (head_dim 512)
+mid-block attention projections run on the wgmma GEMM.  The single-head (head_dim 512)
 mid-block attention is computed per image as S = Q K^T (GEMM, fp32 out), a row softmax
 kernel, and O = P V against V^T, which the V projection produces directly
 (V^T = W_v X^T); the V bias commutes with the softmax average and is folded into the
@@ -214,7 +214,7 @@ class AutoencoderKL(torch.nn.Module):
         d = self.decoder
         dev = d.conv_in.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("AutoencoderKL.decode runs on CUDA (sm_100a) only; there "
+            raise RuntimeError("AutoencoderKL.decode runs on CUDA (sm_90a) only; there "
                                "is no CPU fallback.")
         dt = self.compute_dtype
 
@@ -331,7 +331,7 @@ class AutoencoderKL(torch.nn.Module):
         e = self.encoder
         dev = e.conv_in.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("AutoencoderKL.encode runs on CUDA (sm_100a) only; there is no "
+            raise RuntimeError("AutoencoderKL.encode runs on CUDA (sm_90a) only; there is no "
                                "CPU fallback.")
         dt = self.compute_dtype
 

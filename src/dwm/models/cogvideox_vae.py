@@ -1,4 +1,4 @@
-"""CogVideoX temporal VAE — decode path, B200-native.
+"""CogVideoX temporal VAE — decode path, H100-native.
 
 Mirror of the part of diffusers==0.31.0 `AutoencoderKLCogVideoX` that the reference uses
 on the CTSD hot path (`vae.decode(z / scaling_factor + shift, return_dict=False)[0]`,
@@ -13,12 +13,12 @@ remainder) with the causal-conv caches carried across chunks, so GroupNorm stati
 per chunk (SURVEY.md Appendix A.7).
 
 Execution: activations are channels-last; every causal 3x3x3 convolution and the
-per-frame 3x3 upsampler convolution is the im2col-free tcgen05 kernel
+per-frame 3x3 upsampler convolution is the im2col-free wgmma kernel
 (`dwm_b200_conv`, taps iterated inside the MMA loop, spatial padding = TMA OOB fill,
 causal temporal padding = two cached frames kept in front of each conv input buffer);
 SpatialNorm3D (GroupNorm * conv_y(zq) + conv_b(zq)) + SiLU is one fused pass that emits
 the next convolution's 16-bit input; conv_y / conv_b / conv_shortcut (1x1x1) run on the
-tcgen05 GEMM at latent resolution; residual adds are conv epilogues.
+wgmma GEMM at latent resolution; residual adds are conv epilogues.
 """
 import json
 import math
@@ -174,7 +174,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         else:
             state = torch.load(os.path.join(path, "diffusion_pytorch_model.bin"),
                                map_location="cpu", weights_only=True)
-        # a checkpoint that carries the encoder gets it (validated on B200 against the oracle,
+        # a checkpoint that carries the encoder gets it (validated against the oracle,
         # tests/test_vae_gpu.py::test_encode_matches_oracle), as diffusers' class always does
         has_enc = any(k.startswith("encoder.") for k in state)
         cfg.setdefault("with_encoder", has_enc)
@@ -197,7 +197,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
     def _pack(self):
         dev = self.decoder.conv_in.conv.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("AutoencoderKLCogVideoX.decode runs on CUDA (sm_100a) "
+            raise RuntimeError("AutoencoderKLCogVideoX.decode runs on CUDA (sm_90a) "
                                "only; there is no CPU fallback.")
         dt = self.compute_dtype
 
@@ -323,7 +323,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         e = self.encoder
         dev = e.conv_in.conv.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("AutoencoderKLCogVideoX.encode runs on CUDA (sm_100a) only; "
+            raise RuntimeError("AutoencoderKLCogVideoX.encode runs on CUDA (sm_90a) only; "
                                "there is no CPU fallback.")
         dt = self.compute_dtype
 

@@ -1,4 +1,4 @@
-"""Building blocks grafted into the base diffusion model — B200-native mirror of
+"""Building blocks grafted into the base diffusion model — H100-native mirror of
 reference src/dwm/models/crossview_temporal.py (AlphaBlender :9-72,
 VTSelfAttentionBlock :536-582).
 
@@ -113,7 +113,7 @@ class AlphaBlender(torch.nn.Module):
 class VTSelfAttentionBlock(torch.nn.Module):
     """LN -> GEGLU-FF + res ; LN -> MHSA(+qk RMSNorm) + res ; LN -> GEGLU-FF + res
     (reference crossview_temporal.py:536-582), executed as 3 LayerNorm launches,
-    5 tcgen05 GEMMs with fused epilogues and one gathered-attention launch."""
+    5 wgmma GEMMs with fused epilogues and one gathered-attention launch."""
 
     def __init__(self, dim: int, time_mix_inner_dim: int,
                  num_attention_heads: int, attention_head_dim: int,

@@ -1,4 +1,4 @@
-"""CTSD-3.x MMDiT with cross-view / temporal grafts — B200-native mirror of reference
+"""CTSD-3.x MMDiT with cross-view / temporal grafts — H100-native mirror of reference
 src/dwm/models/crossview_temporal_dit.py:105-630 (`DiTCrossviewTemporalConditionModel`,
 a subclass of diffusers `SD3Transformer2DModel`).
 
@@ -6,7 +6,7 @@ Same constructor kwargs (the JSON config keys), same `forward` signature and ret
 value, same state_dict key names (SURVEY.md Appendix B) — but the forward is a fixed
 sequence of `opendwm_b200` kernel launches over pre-packed 16-bit weights:
 
-  * every Linear (incl. patchify conv, AdaLN linears, FFNs, q/k/v/out) is the tcgen05
+  * every Linear (incl. patchify conv, AdaLN linears, FFNs, q/k/v/out) is the wgmma
     GEMM with a fused epilogue (bias, GELU, GEGLU, per-head RMSNorm, gate*x+residual,
     AlphaBlender);
   * LayerNorm + AdaLN modulation emit the next GEMM operand in one pass;
@@ -268,7 +268,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         dev = self.proj_out.weight.device
         if dev.type != "cuda":
             raise RuntimeError(
-                "DiTCrossviewTemporalConditionModel runs on CUDA (sm_100a) only; "
+                "DiTCrossviewTemporalConditionModel runs on CUDA (sm_90a) only; "
                 "there is no CPU fallback. Move the model to the GPU first.")
         dt = self._dtype()
         D = self.inner_dim

@@ -1,4 +1,4 @@
-"""CTSD-2.1 UNet with cross-view / temporal grafts — B200-native mirror of reference
+"""CTSD-2.1 UNet with cross-view / temporal grafts — H100-native mirror of reference
 src/dwm/models/crossview_temporal_unet.py:355-835 (`UNetCrossviewTemporalConditionModel`,
 a subclass of diffusers `UNetSpatioTemporalConditionModel`) and of the blocks it is made
 of (`ResBlock`, `TransformerModel`, `TemporalBasicTransformerBlock`,
@@ -7,8 +7,8 @@ src/dwm/models/crossview_temporal.py:75-514).
 Same constructor kwargs, forward signature / return value and state_dict key names
 (incl. the SD-2.1 -> SVD key renamer `try_to_convert_state_dict`).  Activations are
 channels-last token matrices `[(b t v) (h w), C]` (fp32 stream, 16-bit GEMM / conv
-operands); every 3x3 convolution is the im2col-free tcgen05 conv, every Linear the
-tcgen05 GEMM, GroupNorm(+SiLU) one fused pass, attention the gathered / tcgen05
+operands); every 3x3 convolution is the im2col-free wgmma conv, every Linear the
+wgmma GEMM, GroupNorm(+SiLU) one fused pass, attention the gathered / wgmma
 attention kernels.  The spatial / cross-view / temporal regroupings are index arithmetic
 inside the attention kernel, exactly as in the DiT mirror.
 """
@@ -272,7 +272,7 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
     def _pack(self):
         dev = self.conv_in.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("UNetCrossviewTemporalConditionModel runs on CUDA (sm_100a) "
+            raise RuntimeError("UNetCrossviewTemporalConditionModel runs on CUDA (sm_90a) "
                                "only; there is no CPU fallback. Move the model to the GPU.")
         dt = self._dtype()
 

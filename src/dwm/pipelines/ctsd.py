@@ -4,7 +4,7 @@ src/dwm/pipelines/ctsd.py: `CrossviewTemporalSD` (ctor :844-1012, condition buil
 and `StreamingCrossviewTemporalSD` (diffusion-forcing FIFO :2010-2277).
 
 Scope (SURVEY.md §8): the denoise loop, its integer timestep-index schedule, CFG
-batching, the model call and the scheduler update run on the B200-native kernels
+batching, the model call and the scheduler update run on the H100-native kernels
 (`model.forward_tokens` + one fused CFG / un-patchify / per-frame-Euler / masked-update
 kernel per step, no host synchronisation inside the loop); the VAE decode runs on the
 mirrored CogVideoX / AutoencoderKL decoders (loaded from `<path>/vae`, or supplied as
@@ -237,7 +237,7 @@ class CrossviewTemporalSD:
         self.output_path = output_path
         if self.device.type != "cuda":
             raise RuntimeError(
-                "dwm.pipelines.ctsd runs on CUDA (sm_100a) only; there is no CPU "
+                "dwm.pipelines.ctsd runs on CUDA (sm_90a) only; there is no CPU "
                 "fallback")
 
         self.generator = torch.Generator()

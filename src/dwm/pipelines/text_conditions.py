@@ -5,7 +5,7 @@ through Hugging Face `transformers`, exactly as in the reference
 (src/dwm/pipelines/ctsd.py:39-83 `flatten_clip_text`, :176-253 the text branch of
 `get_conditions`, :744-805 the SD-3 prompt encoders, :886-948 loading).  This module is the
 thin adapter that lets reference-style batches (`clip_text` = nested prompt lists) drive the
-B200 pipeline when the encoder weights are present; batches that carry pre-encoded
+H100 pipeline when the encoder weights are present; batches that carry pre-encoded
 `text_embeddings` / `pooled_text_embeddings` bypass it.
 """
 import os

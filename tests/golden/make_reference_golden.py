@@ -34,6 +34,7 @@ deterministically (tests/common.py).  tests/test_reference_golden_cpu.py checks 
 restatement against them (bit-exact on the build host; 1e-6 elsewhere), which pins the
 oracle's restatement of OpenDWM's own code.  Usage:  python tests/golden/make_reference_golden.py
 """
+import glob
 import json
 import os
 import sys
@@ -253,7 +254,19 @@ def main():
     with open(os.path.join(OUT, "reference_text_conditions.json"), "w") as f:
         json.dump(text, f, indent=1)
 
-    safetensors.torch.save_file(out, os.path.join(OUT, "reference_outputs.safetensors"))
+    # shards of at most ~900 KB, read back together by tests/test_reference_golden.py
+    shards, size = [{}], 0
+    for k in sorted(out):
+        n = out[k].numel() * out[k].element_size()
+        if size + n > 900_000:
+            shards.append({})
+            size = 0
+        shards[-1][k] = out[k]
+        size += n
+    for old in glob.glob(os.path.join(OUT, "reference_outputs_*.safetensors")):
+        os.remove(old)      # a shorter set of shards must not leave stale keys behind
+    for i, shard in enumerate(shards):
+        safetensors.torch.save_file(shard, os.path.join(OUT, "reference_outputs_%d.safetensors" % i))
     with open(os.path.join(OUT, "reference_autoregressive_traces.json"), "w") as f:
         json.dump(traces, f, indent=1)
     with open(os.path.join(OUT, "reference_outputs.json"), "w") as f:

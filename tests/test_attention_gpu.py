@@ -29,8 +29,8 @@ def _tol(dtype):
 @pytest.fixture(params=[0, 2], ids=["mma", "tc2"])
 def tc_variant(request):
     """Both attention kernels: 0 = attention.cu (mma.sync, gathered addressing), 2 =
-    attention_tc2.cu (tcgen05: two CTAs per SM, O in TMEM with lazy rescale; contiguous and
-    gathered-unit sequences)."""
+    attention_wgmma.cu (warpgroup MMA, S / P / O in registers; contiguous and gathered-unit
+    sequences)."""
     from opendwm_b200 import lib
     lib.set_option("attn_tc", request.param)
     yield request.param
@@ -91,7 +91,7 @@ def test_crossview_rowwise(use_mask, V, W, dtype, tc_variant):
                                       (19, "rowwise", 28), (16, "rowwise", 28), (6, "rowwise", 28)])
 def test_temporal(T, kind, W, tc_variant):
     """Row-wise with W = 28 are the full-size sequences (T x W = 532 / 448 / 168: three group
-    dims, tiles of 4 frames) that take the gathered tcgen05 path."""
+    dims, tiles of 4 frames) that take the gathered wgmma path."""
     from opendwm_b200 import ops
     B, V, H, heads = 2, 2, 2, 2
     S, D, dtype = H * W, heads * 64, torch.bfloat16
@@ -127,7 +127,7 @@ def test_temporal(T, kind, W, tc_variant):
 @pytest.mark.parametrize("seq,N,heads", [(448, 5, 4), (129, 3, 2), (200, 7, 1), (640, 2, 3),
                                          (65, 4, 2), (602, 40, 24)])
 def test_contiguous_sequences_tcgen05(seq, N, heads, dtype, tc_variant):
-    """Contiguous unmasked groups take the tcgen05/TMEM kernel (attention_tc2.cu)."""
+    """Contiguous unmasked groups take the wgmma kernel (attention_wgmma.cu)."""
     from opendwm_b200 import ops
     D = heads * 64
     qkv = _qkv(N * seq, D, dtype, seed=seq)
@@ -142,8 +142,8 @@ def test_contiguous_sequences_tcgen05(seq, N, heads, dtype, tc_variant):
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 def test_growing_logits_exercise_rescale(dtype, tc_variant):
     """Keys of later blocks carry much larger logits, so the running max grows by far more
-    than 2^8 between key blocks (the lazy-rescale branch of attention_tc2.cu) and also by
-    small steps (the no-rescale branch)."""
+    than 2^8 between key blocks and also by small steps: the online-softmax rescale of the
+    running output must stay exact in both regimes."""
     from opendwm_b200 import ops
     N, seq, heads = 3, 602, 2
     D = heads * 64

@@ -62,11 +62,3 @@ def test_workload_blocks_exist_and_match_the_configs_named_in_baseline():
     assert any("ctsd_35_tvae_6views_video_generation_with_layout.json" in c
                for c in base["configs"])
 
-
-def test_traffic_table_is_well_formed():
-    with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-        t = json.load(f)
-    for row in t["kernels"]:
-        assert len(row["shape"]) == 3 and row["dtype"] in ("bf16", "fp16")
-        assert row["dram_read_bytes"] > 0 and row["dram_write_bytes"] > 0
-        assert os.path.exists(os.path.join(ROOT, row["capture"]))

@@ -1,4 +1,4 @@
-"""Parity of the im2col-free tcgen05 convolution against torch conv3d (fp32) on the same
+"""Parity of the im2col-free wgmma convolution against torch conv3d (fp32) on the same
 16-bit inputs: CogVideoX causal 3x3x3, per-frame 1x3x3, 3x3 adapter conv, ragged tiles."""
 import pytest
 import torch
@@ -88,9 +88,10 @@ def test_per_item_residual():
     (1, 1, 299, 130, 128, 320, (1, 3, 3)),  # ragged W tiles, 5 N tiles of 64
 ])
 def test_two_cta_conv_equals_one_cta(shape, epilogue):
-    """Enough pixel tiles (>= 2 x SMs) route the convolution to the cta_group::2 kernel (two
-    pixel tiles per MMA, half a weight slice per CTA); it must agree with the 1-CTA kernel bit
-    for bit (same accumulation order) and with torch."""
+    """Enough pixel tiles (>= 2 x SMs) route the convolution to the kernel for clusters of two
+    CTAs (two pixel tiles sharing each weight slice, half of it loaded by each CTA and
+    multicast); it must agree with the 1-CTA kernel bit for bit (same accumulation order) and
+    with torch."""
     from opendwm_b200 import lib
     lib.set_option("conv_2cta", 1)
     lib.set_option("conv_halo", 0)       # the per-tap pair kernel, not the halo-row one
@@ -117,7 +118,7 @@ def test_two_cta_conv_equals_one_cta(shape, epilogue):
 ])
 def test_halo_row_conv_equals_shifted_patch_kernels(shape, epilogue):
     """kw = 3, W >= 128, C_out tiles <= 128: the halo-row kernel loads each 130-pixel row
-    segment once and feeds the three dw taps through row-shifted UMMA descriptors; it must
+    segment once and feeds the three dw taps through row-shifted wgmma descriptors; it must
     match torch and the per-tap kernels (different tap order: agreement to rounding)."""
     from opendwm_b200 import lib
     tol = 8e-3 if epilogue == "store" else 1e-3

@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 GEMM + fused epilogues (dwm_b200_linear) against a plain
+"""Parity of the wgmma GEMM + fused epilogues (dwm_b200_linear) against a plain
 fp32 PyTorch evaluation of the same math on the same 16-bit inputs."""
 import pytest
 import torch
@@ -8,8 +8,8 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(autouse=True, params=["1cta", "2cta"])
 def gemm_variant(request):
-    """Every test runs on the 1-CTA kernel and on the cta_group::2 cluster kernel
-    (the latter is used for M >= 512)."""
+    """Every test runs on the 1-CTA kernel and on the kernel for clusters of two CTAs that
+    share the weight tile by TMA multicast (the latter is used for M >= 512)."""
     from opendwm_b200 import lib
     lib.set_option("gemm_2cta", 1 if request.param == "2cta" else 0)
     yield
@@ -157,15 +157,17 @@ def test_errors_are_loud():
     (512, 256, 64),            # one tile per cluster
     (3 * 448 + 77, 1536, 256),  # M tail (not a multiple of 32), 6 N-tiles
     (700, 320, 192),           # N % 256 != 0: dead chunks keep the stream in step
-    (148 * 256 + 999, 512, 128),   # > 74 clusters' worth of tiles: multi-tile chunk streams
+    (148 * 256 + 999, 512, 128),   # more tile pairs than clusters: several tiles per persistent CTA
     (5376, 1536, 1536),        # north-star out-proj shape (one frame group)
 ])
 @pytest.mark.parametrize("bn", [256, 128])
 def test_resid_tma_epilogue_equals_register_epilogue(M, N, K, dtype, bn, gemm_variant):
-    """RESID epilogue with the residual tile staged through TMA (load + store, `resid_tma` = 1,
-    2-CTA kernel) against the register/transposing epilogue and against fp32 PyTorch: plain
-    residual, in place, separate output, gate, bias, AlphaBlender; the two kernels must agree
-    to rounding (same operation order, fma contraction aside)."""
+    """RESID epilogue against fp32 PyTorch (plain residual, in place, separate output, gate,
+    bias, AlphaBlender) with the residual / blend rows prefetched into L2 by the TMA unit while
+    the tile's MMAs run (`resid_tma` = 1) on the `bn`-column tile, and bit for bit against the
+    OTHER tile width run without the prefetch: a second kernel instantiation whose epilogue
+    drains differently split chunks must produce the same bits (same K order, explicit
+    roundings in resid_elem / blend_elem)."""
     from opendwm_b200 import ops, lib
     S = 50
     items = (M + S - 1) // S
@@ -184,9 +186,9 @@ def test_resid_tma_epilogue_equals_register_epilogue(M, N, K, dtype, bn, gemm_va
     al = alpha[rows // rpb][:, None]
     ref_blend = al * x + (1 - al) * (resid + z)
 
-    def run(tma):
+    def run(tma, tile_n):
         lib.set_option("resid_tma", tma)
-        lib.set_option("gemm_bn", bn)          # 128: the narrow-tile variant (tail-wave repair)
+        lib.set_option("gemm_bn", tile_n)      # 128: the narrow-tile variant (tail-wave repair)
         try:
             y1 = ops.linear(a, w, b, epilogue=lib.EPI_RESID, resid=resid, gate=gate,
                             rows_per_item=S)
@@ -204,7 +206,7 @@ def test_resid_tma_epilogue_equals_register_epilogue(M, N, K, dtype, bn, gemm_va
         finally:
             lib.set_option("resid_tma", 1)
             lib.set_option("gemm_bn", 0)
-    new, old = run(1), run(0)
+    new, old = run(1, bn), run(0, 384 - bn)
     for got, ref in zip(new, (ref_gate, ref_gate, ref_blend, ref_blend, resid + z - b)):
         assert _relerr(got, ref) < 2e-5
     for g, o in zip(new, old):      # explicit roundings (resid_elem / blend_elem): same bits

@@ -1,4 +1,4 @@
-"""Parity of the B200-native DiT forward against the fp32 oracle (same state_dict,
+"""Parity of the H100-native DiT forward against the fp32 oracle (same state_dict,
 same seeded inputs).  Metric: max|y - ref| / max|ref| (SURVEY.md §7 tolerance policy).
 Stated tolerances: bf16 operands 2e-2, fp16 operands 4e-3 for this 4-layer model
 (16-bit GEMM operands, fp32 accumulation / statistics / residual stream)."""

@@ -25,8 +25,12 @@ SD21 = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012,
 
 @pytest.fixture(scope="module")
 def golden():
+    import glob
     import safetensors.torch
-    return safetensors.torch.load_file(os.path.join(HERE, "golden", "reference_outputs.safetensors"))
+    out = {}
+    for f in sorted(glob.glob(os.path.join(HERE, "golden", "reference_outputs_*.safetensors"))):
+        out.update(safetensors.torch.load_file(f))
+    return out
 
 
 def _rel(a, b):

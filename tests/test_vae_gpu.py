@@ -1,4 +1,4 @@
-"""Parity of the B200-native CogVideoX decoder against the fp32 oracle restatement:
+"""Parity of the H100-native CogVideoX decoder against the fp32 oracle restatement:
 single chunk, chunked decode with causal caches (odd and even frame counts), the
 diffusion-forcing single-frame decode, and state_dict key parity."""
 import pytest

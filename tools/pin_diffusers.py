@@ -29,6 +29,15 @@ def _rel(a, b):
     return ((a.double() - b.double()).abs().max() / b.double().abs().max().clamp_min(1e-30)).item()
 
 
+def _load_shards(d):
+    import glob
+    import safetensors.torch
+    out = {}
+    for f in sorted(glob.glob(os.path.join(d, "reference_outputs_*.safetensors"))):
+        out.update(safetensors.torch.load_file(f))
+    return out
+
+
 def main():
     try:
         import diffusers
@@ -53,9 +62,8 @@ def main():
         subprocess.run([sys.executable, os.path.join(ROOT, "tests", "golden",
                                                      "make_reference_golden.py")],
                        check=True, env=env)
-        new = safetensors.torch.load_file(os.path.join(tmp, "reference_outputs.safetensors"))
-    old = safetensors.torch.load_file(
-        os.path.join(ROOT, "tests", "golden", "reference_outputs.safetensors"))
+        new = _load_shards(tmp)
+    old = _load_shards(os.path.join(ROOT, "tests", "golden"))
     for k in sorted(old):
         if k not in new:
             print("MISSING", k)

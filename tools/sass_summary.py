@@ -1,8 +1,8 @@
 """Per-kernel counts of the SASS mnemonics that show which hardware path a kernel uses
-(tcgen05 = UTC*MMA, TMEM = LDTM/STTM, TMA = UTMALDG / UTMASTG / UBLKCP / UTMAPF, legacy tensor
-path = HMMA), from `cuobjdump -sass` of the in-tree library.  Runs without a GPU.
+(warpgroup MMA = HGMMA, TMA = UTMALDG / UTMASTG / UBLKCP / UTMAPF, mma.sync tensor path =
+HMMA), from `cuobjdump -sass` of the in-tree library.  Runs without a GPU.
 
-    python tools/sass_summary.py > profiles/r02_sass_summary.txt
+    python tools/sass_summary.py
 """
 import collections
 import os
@@ -12,9 +12,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "opendwm_b200", "libdwm_b200.so")
-PATTERNS = ["UTCHMMA", "UTCHMMA.2CTA", "LDTM", "STTM", "UTMALDG", "UTMALDG.2CTA", "UTMASTG",
-            "UTMAPF", "UBLKCP", "UBLKPF", "UTCBAR", "SYNCS", "HMMA", "LDSM", "LDGSTS", "MUFU.EX2",
-            "RED.", "ATOM"]
+PATTERNS = ["HGMMA", "WARPGROUP.ARRIVE", "UTMALDG", "UTMASTG", "UTMAPF", "UBLKCP", "UBLKPF",
+            "SYNCS", "USETMAXREG", "HMMA", "LDSM", "LDGSTS", "MUFU.EX2", "RED.", "ATOM"]
 
 
 def main():
@@ -45,7 +44,7 @@ def main():
             if hit:
                 kernels[name][p] += 1
     print("SASS mnemonic counts per kernel of opendwm_b200/libdwm_b200.so (cuobjdump -sass, "
-          "sm_100a)\n")
+          "sm_90a)\n")
     cols = [p for p in PATTERNS if any(k[p] for k in kernels.values())]
     width = max(len(n) for n in kernels) + 2
     print("kernel".ljust(width) + "".join(c.rjust(max(9, len(c) + 1)) for c in cols))
@@ -56,7 +55,7 @@ def main():
         print(n.ljust(width) + "".join(str(c[p] or ".").rjust(max(9, len(p) + 1)) for p in cols))
         total.update(c)
     print("\nTOTAL".ljust(width + 1) + "".join(str(total[p]).rjust(max(9, len(p) + 1)) for p in cols))
-    print("\nUTCHMMA = tcgen05.mma (kind::f16), .2CTA = cta_group::2; LDTM/STTM = tcgen05.ld/st; "
+    print("\nHGMMA = wgmma.mma_async, WARPGROUP.ARRIVE = wgmma.fence, USETMAXREG = setmaxnreg; "
           "UTMALDG/UTMASTG = cp.async.bulk.tensor load/store (TMA), UTMAPF = TMA L2 prefetch, "
           "UBLKCP/UBLKPF = cp.async.bulk copy / prefetch; HMMA + LDSM = mma.sync path "
           "(gathered attention kernel for short / separate-KV sequences only).")

@@ -35,7 +35,7 @@ def main():
     cases = [(8, "pointwise"), (5, "pointwise"), (11, "pointwise"), (19, "pointwise"),
              (19, "rowwise"), (5, "rowwise")]
     cases = [c for c in cases if c[0] >= t_ways]
-    # row-wise sequences longer than 64 take the tcgen05 kernel when unsharded and the
+    # row-wise sequences longer than 64 take the wgmma kernel when unsharded and the
     # separate-K,V mma.sync kernel when sharded; with attn_tc = 0 both runs use the same kernel
     # and the comparison is bit for bit
     lib.set_option("attn_tc", 0)
