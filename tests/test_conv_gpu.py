@@ -52,6 +52,7 @@ def test_causal_conv3d_3x3x3(dtype):
     (2, 1, 8, 14, 64, 320, (1, 3, 3)),      # UNet widths: 5 tiles of 64
     (1, 1, 8, 14, 320, 640, (1, 3, 3)),     # 5 tiles of 128, C_in 320 = 5 k-blocks
     (1, 1, 4, 7, 128, 1280, (1, 3, 3)),     # 5 tiles of 256
+    (2, 4, 1, 112, 64, 128, (3, 1, 1)),     # temporal ResBlock conv: 3 frame taps, no padding
 ])
 def test_shapes(shape):
     err = _case(*shape, torch.bfloat16)
@@ -133,3 +134,47 @@ def test_halo_row_conv_equals_shifted_patch_kernels(shape, epilogue):
         lib.set_option("conv_halo", 1)
     assert eh < tol and e2 < tol, (eh, e2)
     assert ((yh - y2).abs().max() / y2.abs().max()).item() < (2e-3 if epilogue == "store" else 2e-5)
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+@pytest.mark.parametrize("C", [320, 640])
+@pytest.mark.parametrize("S", [112, 1792])
+def test_temporal_resblock_convs(S, C, dtype):
+    """The two (3,1,1) convolutions of the UNet TemporalResnetBlock on `(b v)` volumes
+    [B*V, T+2, 1, S, C] with a zero frame at both ends: (i) + one temb row per (b, v, t) item;
+    (ii) + the block input as residual, then the AlphaBlender against that same tensor,
+    out = alpha[b] * x + (1 - alpha[b]) * (conv + bias + x).  S = 1792 (SD-2.1 level 0 at
+    256 x 448) has enough pixel tiles for the 2-CTA kernel, which must give the bits of the
+    1-CTA kernel."""
+    from opendwm_b200 import ops, lib
+    B, V, T = 2, 3, 8
+    g = torch.Generator().manual_seed(S + C)
+    x = torch.zeros(B * V, T + 2, 1, S, C, dtype=dtype, device="cuda")
+    x[:, 1:T + 1] = torch.randn(B * V, T, 1, S, C, generator=g).to(dtype).cuda()
+    wt = (torch.randn(C, C, 3, 1, 1, generator=g) * (3 * C) ** -0.5).to(dtype).cuda()
+    b = torch.randn(C, generator=g).cuda()
+    temb = torch.randn(B * V * T, C, generator=g).cuda()
+    xr = torch.randn(B * V * T * S, C, generator=g).cuda()
+    alpha = torch.tensor([0.3, 0.8], device="cuda")
+    conv = torch.nn.functional.conv3d(x.float().permute(0, 4, 1, 2, 3), wt.float(), b)
+    conv = conv.permute(0, 2, 3, 4, 1).reshape(-1, C)               # rows (b v, t, s)
+    ref1 = conv + temb.repeat_interleave(S, 0)
+    a = alpha.repeat_interleave(V * T * S)[:, None]
+    ref2 = a * xr + (1 - a) * (conv + xr)
+    wp = ops.pack_conv_weight(wt, dtype)
+    outs = {}
+    try:
+        for two in (1, 0):
+            lib.set_option("conv_2cta", two)
+            y1 = ops.conv(x, wp, b, kernel=(3, 1, 1), epilogue=lib.EPI_RESID, resid=temb,
+                          resid_rows_per_item=S)
+            y2 = ops.conv(x, wp, b, kernel=(3, 1, 1), epilogue=lib.EPI_RESID, resid=xr,
+                          blend_x=xr, alpha=alpha, rows_per_batch=V * T * S)
+            outs[two] = (y1, y2)
+    finally:
+        lib.set_option("conv_2cta", 1)
+    for name, y, ref in zip(("temb", "blend"), outs[1], (ref1, ref2)):
+        err = ((y - ref).abs().max() / ref.abs().max()).item()
+        assert err < 1e-3, (name, err)
+    for y2, y1 in zip(outs[1], outs[0]):
+        assert torch.equal(y2, y1)

@@ -49,17 +49,18 @@ def test_store(M, N, K, dtype):
     torch.testing.assert_close(y2, ref, rtol=1e-3, atol=1e-3 * ref.abs().max().item())
 
 
-@pytest.mark.parametrize("act", ["gelu_tanh", "gelu_erf", "silu"])
+@pytest.mark.parametrize("act", ["gelu_tanh", "gelu_erf", "silu", "relu"])
 def test_activation(act):
     from opendwm_b200 import ops, lib
-    code = {"gelu_tanh": lib.ACT_GELU_TANH, "gelu_erf": lib.ACT_GELU_ERF, "silu": lib.ACT_SILU}[act]
+    code = {"gelu_tanh": lib.ACT_GELU_TANH, "gelu_erf": lib.ACT_GELU_ERF, "silu": lib.ACT_SILU,
+            "relu": lib.ACT_RELU}[act]
     a = _mk((300, 512), torch.bfloat16, seed=1)
     w = _mk((1024, 512), torch.bfloat16, 0.05, seed=2)
     b = _mk((1024,), torch.float32, seed=3)
     z = a.float() @ w.float().t() + b
     ref = {"gelu_tanh": lambda t: torch.nn.functional.gelu(t, approximate="tanh"),
            "gelu_erf": torch.nn.functional.gelu,
-           "silu": torch.nn.functional.silu}[act](z)
+           "silu": torch.nn.functional.silu, "relu": torch.relu}[act](z)
     y = ops.linear(a, w, b, epilogue=lib.EPI_F32, act=code)
     assert _relerr(y, ref) < 1e-5
     y16 = ops.linear(a, w, b, act=code)

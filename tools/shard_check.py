@@ -31,11 +31,12 @@ def main():
     use_cfg = os.environ.get("SHARD_CFG", "1") != "0"
     t_ways = world // (2 if (use_cfg and world >= 2) else 1)
     # (frames, temporal attention type): 8 = even shards; 5 / 11 / 19 = the uneven shards of
-    # BASELINE configs 5 and 3 (19 with row-wise temporal attention as in config 3)
+    # BASELINE configs 5 and 3 (19 with row-wise temporal attention as in config 3); full
+    # temporal attention on even and uneven shards
     cases = [(8, "pointwise"), (5, "pointwise"), (11, "pointwise"), (19, "pointwise"),
-             (19, "rowwise"), (5, "rowwise")]
+             (19, "rowwise"), (5, "rowwise"), (8, "full"), (5, "full")]
     cases = [c for c in cases if c[0] >= t_ways]
-    # row-wise sequences longer than 64 take the wgmma kernel when unsharded and the
+    # row-wise / full sequences longer than 64 take the wgmma kernel when unsharded and the
     # separate-K,V mma.sync kernel when sharded; with attn_tc = 0 both runs use the same kernel
     # and the comparison is bit for bit
     lib.set_option("attn_tc", 0)
