@@ -15,6 +15,7 @@
  *  - all pointers are DEVICE pointers owned by the caller (PyTorch); nothing is
  *    allocated here.  Launches are asynchronous on `stream`.
  *  - 16-bit activations/weights are bf16 (DWM_BF16) or fp16 (DWM_F16);
+ *    opt-in 8-bit GEMM operands are E4M3 (DWM_E4M3) with one fp32 scale per row;
  *    biases, norm weights, modulation vectors, residual streams are fp32.
  *  - there is NO CPU fallback: calling these without a Hopper (sm_90a) GPU fails.
  */
@@ -30,7 +31,7 @@ extern "C" {
 
 typedef void* dwm_stream_t; /* cudaStream_t */
 
-enum dwm_dtype { DWM_BF16 = 0, DWM_F16 = 1, DWM_F32 = 2 };
+enum dwm_dtype { DWM_BF16 = 0, DWM_F16 = 1, DWM_F32 = 2, DWM_E4M3 = 3 };
 enum dwm_act { DWM_ACT_NONE = 0, DWM_ACT_GELU_TANH = 1, DWM_ACT_GELU_ERF = 2, DWM_ACT_SILU = 3, DWM_ACT_RELU = 4 };
 
 /* Epilogues of dwm_b200_linear (all fused into the wgmma GEMM kernel). */
@@ -98,6 +99,14 @@ typedef struct dwm_linear_args {
    * all-gather by one kernel. */
   void* peer_out[8];
   int n_peer_out;
+  /* FP8 (dtype == DWM_E4M3): A and W are E4M3 with row scales, a_scale fp32 [M] and
+   * w_scale fp32 [N] (one per weight row = output channel, in packed row order).  The fp32
+   * accumulator of A8 . W8^T is multiplied by a_scale[m] * w_scale[n] before the bias; the
+   * epilogue then runs as for 16-bit operands, with out_dtype (DWM_BF16 / DWM_F16) the type
+   * of its 16-bit outputs.  K, lda and ldw must be multiples of 16. */
+  const float* a_scale;
+  const float* w_scale;
+  int out_dtype;
 } dwm_linear_args;
 
 const char* dwm_b200_version(void);
@@ -211,9 +220,22 @@ typedef struct dwm_layernorm_args {
   void* out2;
   int64_t ldo2;
   int dtype;
+  /* dtype == DWM_E4M3: out (and out2) are E4M3; each row is quantized from its fp32
+   * modulated value with scale amax(|row|) / 448, written to out_scale[m] (out2_scale[m]). */
+  float* out_scale;
+  float* out2_scale;
 } dwm_layernorm_args;
 
 int dwm_b200_layernorm(const dwm_layernorm_args* args, dwm_stream_t stream);
+
+/* Row-wise E4M3 quantization of a GEMM operand: x [M, K] (dtype DWM_BF16 / DWM_F16 / DWM_F32,
+ * row pitch ld) -> out E4M3 [M, K] (pitch ldo bytes) and scale fp32 [M].  Per row:
+ * amax = max |x|; amax == 0 -> scale 1, q = 0; otherwise inv = 448 / amax,
+ * q = cvt.rn.satfinite.e4m3(x * inv), scale = amax / 448 (IEEE fp32 divisions).
+ * K must be a multiple of 16.  Feeds the FP8 down / out projections (GELU, GEGLU and
+ * attention outputs) and packs FP8 weights (one scale per output channel). */
+int dwm_b200_quantize_rows(const void* x, int64_t M, int64_t K, int64_t ld, int dtype, void* out,
+                           int64_t ldo, float* scale, dwm_stream_t stream);
 
 /* out16[i] = act(in32[i]) over n elements: SiLU(temb) feeding the AdaLayerNormZero linears of
  * the joint blocks (called at crossview_temporal_dit.py:517-521) and the UNet ResBlock

@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -274,6 +275,25 @@ __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// ---- E4M3 row quantization ------------------------------------------------------
+// One recipe everywhere (GEMM operands and weights): amax == 0 -> scale 1, q = 0; otherwise
+// inv = 448 / amax, q = cvt.rn.satfinite.e4m3(x * inv), scale = amax / 448, IEEE divisions.
+constexpr float kE4M3Max = 448.f;
+__device__ __forceinline__ float e4m3_inv(float amax) { return amax > 0.f ? __fdiv_rn(kE4M3Max, amax) : 0.f; }
+__device__ __forceinline__ float e4m3_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, kE4M3Max) : 1.f; }
+// four values * inv -> four E4M3 bytes, the first in the lowest byte
+__device__ __forceinline__ uint32_t e4m3x4(float a, float b, float c, float d, float inv) {
+  uint16_t lo, hi;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(__fmul_rn(b, inv)), "f"(__fmul_rn(a, inv)));
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(__fmul_rn(d, inv)), "f"(__fmul_rn(c, inv)));
+  return static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
 }
 #endif  // __CUDACC__
 

@@ -1,13 +1,16 @@
 // Persistent warp-specialised wgmma GEMM with fused epilogues (sm_90a).
 //
 //   D[M,N] = A[M,K] · W[N,K]^T     A, W 16-bit (bf16/fp16), fp32 accumulation in registers
+//   FP8:   D[M,N] = a_scale[M] w_scale[N] (A8[M,K] · W8[N,K]^T)  with E4M3 operands (opt-in)
 //
 // Roles (384 threads, one CTA per SM, persistent over 128 x NT output tiles):
 //   warpgroup 0    TMA producer (one elected thread): 128x64 A tile + NTx64 W tile per k-block
 //                  into a 4-stage 128B-swizzled shared-memory ring (mbarrier tx-count completion);
 //                  runs ahead into the next tile while the consumers drain the current one
-//   warpgroups 1-2 consumers: each issues wgmma m64nNTk16 for its 64 rows of the tile and
-//                  then applies the fused epilogue straight from its register fragment
+//   warpgroups 1-2 consumers: each issues wgmma m64nNTk16 (k32 for E4M3) for its 64 rows of
+//                  the tile and then applies the fused epilogue straight from its register
+//                  fragment (E4M3: after scaling it by the row and channel scales)
+// A stage is 128 bytes of K per row in either case: 64 16-bit or 128 E4M3 elements.
 // NT = 256 (the widest wgmma; 128 accumulator registers per thread) unless a 128-wide tile
 // gives the last wave fewer idle SMs.
 //
@@ -36,12 +39,14 @@ struct GemmCfg {
 // the consumers of BOTH CTAs have released it (the peer writes into it too).  An odd number
 // of M tiles gives the last pair a dummy tile: its A loads are out of bounds (zero fill) and
 // its rows are never stored.  Both variants accumulate in the same order: same bits.
-template <typename T, int EPI, int NT, int CL>
+// TA: operand type (bf16 / fp16 / E4M3); T: type of the 16-bit outputs (TA unless E4M3).
+template <typename TA, typename T, int EPI, int NT, int CL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                       const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
                       EpiParams p) {
   constexpr int B_STAGE_BYTES = GemmCfg<NT>::kBStageBytes;
+  constexpr int BKE = BK * 2 / static_cast<int>(sizeof(TA));   // K elements per stage
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled TMA / wgmma tiles need 1024-byte alignment.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -59,7 +64,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 
   const int m_blocks = (M + BM - 1) / BM;
   const int n_blocks = (N + NT - 1) / NT;
-  const int k_blocks = (K + BK - 1) / BK;
+  const int k_blocks = (K + BKE - 1) / BKE;
   const int num_tiles = ((m_blocks + CL - 1) / CL) * n_blocks;   // CL vertically adjacent tiles each
   const int first = static_cast<int>(blockIdx.x) / CL, step = static_cast<int>(gridDim.x) / CL;
 
@@ -86,13 +91,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         for (int kb = 0; kb < k_blocks; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_expect_tx(&full_bar[stage], A_STAGE_BYTES + B_STAGE_BYTES);
-          tma_load_2d(&tmap_a, &full_bar[stage], smem_a + stage * A_STAGE_BYTES, kb * BK,
+          tma_load_2d(&tmap_a, &full_bar[stage], smem_a + stage * A_STAGE_BYTES, kb * BKE,
                       m_blk * BM, kEvictNormal);
           if constexpr (CL == 2) {
             tma_load_2d_mc(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES + rank * (B_STAGE_BYTES / 2),
-                           kb * BK, n_blk * NT + static_cast<int>(rank) * (NT / 2), 0x3, kEvictLast);
+                           kb * BKE, n_blk * NT + static_cast<int>(rank) * (NT / 2), 0x3, kEvictLast);
           } else {
-            tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES, kb * BK,
+            tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES, kb * BKE,
                         n_blk * NT, kEvictLast);
           }
           if (++stage == STAGES) {
@@ -117,8 +122,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       const int t = threadIdx.x & 127;
       prefetch_resid_tile<EPI, NT>(p, m_blk * BM + cw * 64 + (t >> 1), M, n_blk * NT, N, t & 1);
       float acc[NT / 2];
-      wg_mainloop<T, NT, CL>(acc, smem_a, A_STAGE_BYTES, cw * 64 * 128, smem_b, B_STAGE_BYTES, full_bar,
-                             empty_bar, STAGES, k_blocks, stage, phase, lane, rank ^ 1u);
+      wg_mainloop<TA, NT, CL>(acc, smem_a, A_STAGE_BYTES, cw * 64 * 128, smem_b, B_STAGE_BYTES, full_bar,
+                              empty_bar, STAGES, k_blocks, stage, phase, lane, rank ^ 1u);
+      if constexpr (sizeof(TA) == 1)
+        dequant_frag<NT>(acc, p.a_scale, p.w_scale, m_blk * BM + wrow, M, n_blk * NT, N, lane);
       drain_tile<T, EPI, NT>(acc, stg, m_blk * BM, wrow, M, n_blk * NT, N, p, lane);
     }
   }
@@ -128,12 +135,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 
 int g_resid_tma = 1;   // option "resid_tma": L2 prefetch of the RESID operands by the TMA unit
 
-template <typename T, int EPI, int NT, int CL>
+template <typename TA, typename T, int EPI, int NT, int CL>
 static int launch_gemm(const dwm_linear_args* a, cudaStream_t stream) {
+  constexpr int eb = static_cast<int>(sizeof(TA));
   CUtensorMap ta, tb;
-  int rc = make_tmap_2d(&ta, a->A, a->M, a->K, a->lda, BM, BK, 2);
+  int rc = make_tmap_2d(&ta, a->A, a->M, a->K, a->lda, BM, BK * 2 / eb, eb);
   if (rc) return rc;
-  rc = make_tmap_2d(&tb, a->W, a->N, a->K, a->ldw, NT / CL, BK, 2);
+  rc = make_tmap_2d(&tb, a->W, a->N, a->K, a->ldw, NT / CL, BK * 2 / eb, eb);
   if (rc) return rc;
 
   EpiParams p;
@@ -141,7 +149,7 @@ static int launch_gemm(const dwm_linear_args* a, cudaStream_t stream) {
   p.resid_prefetch = g_resid_tma;
 
   constexpr int smem_bytes = GemmCfg<NT>::kSmemBytes;
-  auto kern = gemm_wgmma_kernel<T, EPI, NT, CL>;
+  auto kern = gemm_wgmma_kernel<TA, T, EPI, NT, CL>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     DWM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -178,22 +186,30 @@ static int pick_tile_n(const dwm_linear_args* a, int cl) {
   return cost128 < cost256 ? 128 : 256;
 }
 
-template <typename T, int EPI, int CL>
+template <typename TA, typename T, int EPI, int CL>
 static int launch_pick_n(const dwm_linear_args* a, cudaStream_t s) {
-  if (pick_tile_n(a, CL) == 128) return launch_gemm<T, EPI, 128, CL>(a, s);
-  return launch_gemm<T, EPI, 256, CL>(a, s);
+  if (pick_tile_n(a, CL) == 128) return launch_gemm<TA, T, EPI, 128, CL>(a, s);
+  return launch_gemm<TA, T, EPI, 256, CL>(a, s);
 }
 
-template <typename T, int CL>
+// TF: the 16-bit type named in the kernel of the fp32-output epilogues, which never use it.
+// 16-bit operands keep TF = T; E4M3 operands share one instantiation between both out_dtypes.
+template <typename TA, typename T, int CL, typename TF = T>
 static int dispatch_epi(const dwm_linear_args* a, cudaStream_t s) {
   switch (a->epilogue) {
-    case DWM_EPI_STORE: return launch_pick_n<T, DWM_EPI_STORE, CL>(a, s);
-    case DWM_EPI_GEGLU: return launch_gemm<T, DWM_EPI_GEGLU, 256, CL>(a, s);
-    case DWM_EPI_QKNORM: return launch_pick_n<T, DWM_EPI_QKNORM, CL>(a, s);
-    case DWM_EPI_RESID: return launch_pick_n<T, DWM_EPI_RESID, CL>(a, s);
-    case DWM_EPI_F32: return launch_pick_n<T, DWM_EPI_F32, CL>(a, s);
+    case DWM_EPI_STORE: return launch_pick_n<TA, T, DWM_EPI_STORE, CL>(a, s);
+    case DWM_EPI_GEGLU: return launch_gemm<TA, T, DWM_EPI_GEGLU, 256, CL>(a, s);
+    case DWM_EPI_QKNORM: return launch_pick_n<TA, T, DWM_EPI_QKNORM, CL>(a, s);
+    case DWM_EPI_RESID: return launch_pick_n<TA, TF, DWM_EPI_RESID, CL>(a, s);
+    case DWM_EPI_F32: return launch_pick_n<TA, TF, DWM_EPI_F32, CL>(a, s);
     default: set_last_error("dwm_b200_linear: unknown epilogue %d", a->epilogue); return -1;
   }
+}
+
+template <int CL>
+static int dispatch_e4m3(const dwm_linear_args* a, cudaStream_t s) {
+  if (a->out_dtype == DWM_BF16) return dispatch_epi<__nv_fp8_e4m3, __nv_bfloat16, CL>(a, s);
+  return dispatch_epi<__nv_fp8_e4m3, __half, CL, __nv_bfloat16>(a, s);
 }
 
 }  // namespace dwm
@@ -225,6 +241,16 @@ extern "C" int dwm_b200_linear(const dwm_linear_args* a, dwm_stream_t stream) {
   DWM_REQUIRE(a->K % 8 == 0 && a->lda % 8 == 0 && a->ldw % 8 == 0,
               "dwm_b200_linear: K, lda, ldw must be multiples of 8 (16-byte TMA pitch); got %lld %lld %lld",
               (long long)a->K, (long long)a->lda, (long long)a->ldw);
+  if (a->dtype == DWM_E4M3) {
+    DWM_REQUIRE(a->K % 16 == 0 && a->lda % 16 == 0 && a->ldw % 16 == 0,
+                "dwm_b200_linear: E4M3 needs K, lda, ldw multiples of 16 (16-byte TMA pitch); got %lld %lld %lld",
+                (long long)a->K, (long long)a->lda, (long long)a->ldw);
+    DWM_REQUIRE(a->a_scale && a->w_scale, "dwm_b200_linear: E4M3 operands need a_scale and w_scale");
+    DWM_REQUIRE(a->out_dtype == DWM_BF16 || a->out_dtype == DWM_F16,
+                "dwm_b200_linear: E4M3 operands need out_dtype DWM_BF16 or DWM_F16, got %d", a->out_dtype);
+    DWM_REQUIRE((reinterpret_cast<uintptr_t>(a->w_scale) & 7) == 0,
+                "dwm_b200_linear: w_scale must be 8-byte aligned");
+  }
   DWM_REQUIRE((reinterpret_cast<uintptr_t>(a->A) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(a->W) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(a->out) & 15) == 0,
@@ -251,8 +277,10 @@ extern "C" int dwm_b200_linear(const dwm_linear_args* a, dwm_stream_t stream) {
   }
   // pairs pay off once there are enough 128-row tiles to give both CTAs of a cluster work
   const bool pair = g_gemm_2cta == 1 && a->M >= 512;
-  if (a->dtype == DWM_BF16) return pair ? dispatch_epi<__nv_bfloat16, 2>(a, s) : dispatch_epi<__nv_bfloat16, 1>(a, s);
-  if (a->dtype == DWM_F16) return pair ? dispatch_epi<__half, 2>(a, s) : dispatch_epi<__half, 1>(a, s);
-  set_last_error("dwm_b200_linear: dtype must be DWM_BF16 or DWM_F16, got %d", a->dtype);
+  if (a->dtype == DWM_BF16)
+    return pair ? dispatch_epi<__nv_bfloat16, __nv_bfloat16, 2>(a, s) : dispatch_epi<__nv_bfloat16, __nv_bfloat16, 1>(a, s);
+  if (a->dtype == DWM_F16) return pair ? dispatch_epi<__half, __half, 2>(a, s) : dispatch_epi<__half, __half, 1>(a, s);
+  if (a->dtype == DWM_E4M3) return pair ? dispatch_e4m3<2>(a, s) : dispatch_e4m3<1>(a, s);
+  set_last_error("dwm_b200_linear: dtype must be DWM_BF16, DWM_F16 or DWM_E4M3, got %d", a->dtype);
   return -1;
 }

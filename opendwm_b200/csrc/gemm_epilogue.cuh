@@ -8,7 +8,7 @@
 namespace dwm {
 
 constexpr int BM = 128;   // accumulator rows per CTA: two consumer warpgroups x 64 rows
-constexpr int BK = 64;    // one 128-byte swizzle atom of 16-bit K per stage
+constexpr int BK = 64;    // one 128-byte swizzle atom of 16-bit K per stage (128 E4M3 elements)
 constexpr int WG_K = 16;
 constexpr int CONSUMER_WGS = 2;
 constexpr int GEMM_THREADS = 128 * (1 + CONSUMER_WGS);   // warpgroup 0: TMA producer
@@ -40,6 +40,8 @@ struct EpiParams {
   void* peer_out[8];
   int n_peers;
   int resid_prefetch;   // RESID: L2 prefetch of the tile's residual / blend rows by the TMA unit
+  const float* a_scale;  // FP8 operands: row scales of A [M] and of W [N]
+  const float* w_scale;
 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -326,12 +328,46 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
   }
 }
 
+// FP8 operands: acc[r, n] *= a_scale[m] * w_scale[n] over the fragment of this warp's 16 rows
+// (first global row m0), before the epilogue adds the bias.  Rows >= M (tile padding) and
+// columns >= N are scaled by 0 so that no scale is read out of bounds.  The product of the two
+// scales is rounded once and applied with one rounded multiply, whatever the tile shape.
+template <int NT>
+__device__ __forceinline__ void dequant_frag(float (&acc)[NT / 2], const float* a_scale, const float* w_scale,
+                                             int m0, int M, int n_tile0, int N, int lane) {
+  const int r = m0 + (lane >> 2);
+  const float s_lo = r < M ? __ldg(a_scale + r) : 0.f;
+  const float s_hi = r + 8 < M ? __ldg(a_scale + r + 8) : 0.f;
+  // groups of 8 column pairs: the compiler barrier keeps the next group's scale loads from
+  // being hoisted next to the 128 live accumulators (which would spill)
+#pragma unroll
+  for (int g = 0; g < NT / 64; ++g) {
+    float2 w[8];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int col = n_tile0 + 8 * (8 * g + jj) + 2 * (lane & 3);
+      w[jj] = col < N ? __ldg(reinterpret_cast<const float2*>(w_scale + col)) : make_float2(0.f, 0.f);
+    }
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int j = 8 * g + jj;
+      acc[4 * j + 0] = __fmul_rn(acc[4 * j + 0], __fmul_rn(s_lo, w[jj].x));
+      acc[4 * j + 1] = __fmul_rn(acc[4 * j + 1], __fmul_rn(s_lo, w[jj].y));
+      acc[4 * j + 2] = __fmul_rn(acc[4 * j + 2], __fmul_rn(s_hi, w[jj].x));
+      acc[4 * j + 3] = __fmul_rn(acc[4 * j + 3], __fmul_rn(s_hi, w[jj].y));
+    }
+    asm volatile("" ::: "memory");
+  }
+}
+
 // One output tile of one consumer warpgroup: acc[64 x NT] = sum over k_iters stages and TAPS
 // taps of A[64 rows at a_row_off (+ t rows for tap t)] . B[NT rows of tap t]^T.  TAPS = 3 is
 // the halo-row convolution: the three dw taps read row-shifted views of one A tile.  Every stage
 // is released (one arrive per consumer warp, on this CTA's barrier and, in a cluster of two
 // that shares the B tile by multicast, on the peer's) as soon as the wgmma that read it has
-// completed; one wgmma group stays in flight.
+// completed; one wgmma group stays in flight.  T is the operand type: a 128-byte K row of a
+// stage is four k16 MMAs of 16-bit or four k32 MMAs of E4M3 elements, with the same descriptor
+// steps.
 template <typename T, int NT, int CL = 1, int TAPS = 1>
 __device__ __forceinline__ void wg_mainloop(float (&acc)[NT / 2], const uint8_t* smem_a, int a_stage_bytes,
                                             int a_row_off_bytes, const uint8_t* smem_b, int b_stage_bytes,
@@ -440,6 +476,8 @@ inline void fill_epi_params(EpiParams& p, const dwm_linear_args* a) {
   p.n_peers = a->n_peer_out;
   p.resid_prefetch = 1;
   for (int i = 0; i < 8; ++i) p.peer_out[i] = i < a->n_peer_out ? a->peer_out[i] : nullptr;
+  p.a_scale = a->a_scale;
+  p.w_scale = a->w_scale;
 }
 
 }  // namespace dwm

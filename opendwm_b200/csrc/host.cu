@@ -102,8 +102,10 @@ static int encode_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uin
   cuuint64_t gstride[1] = {ld * static_cast<uint64_t>(elem_bytes)};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                           : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  // the element type only sets the element size (copies are bitwise; OOB fill is zero bytes)
+  CUtensorMapDataType dt = elem_bytes == 2   ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                           : elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                             : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = fn(map, dt, 2, const_cast<void*>(base), gdim, gstride, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

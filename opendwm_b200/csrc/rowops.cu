@@ -1,6 +1,7 @@
 // Memory-bound row / elementwise kernels of the CTSD step (sm_90a): LayerNorm with
-// AdaLN modulation (emits the 16-bit GEMM operand), activation casts, sinusoidal
-// embeddings, patchify, and the fused CFG + un-patchify + per-frame Euler update.
+// AdaLN modulation (emits the 16-bit or row-scaled E4M3 GEMM operand), E4M3 row quantization,
+// activation casts, sinusoidal embeddings, patchify, and the fused CFG + un-patchify +
+// per-frame Euler update.
 // All are single-pass over HBM with 128-bit accesses.
 #include "common.cuh"
 #include "../../include/dwm_b200.h"
@@ -18,12 +19,14 @@ struct LnParams {
   const float* weight; const float* bias; float eps;
   const float* shift; const float* scale; const float* shift2; const float* scale2; long long mod_ld;
   void* out; long long ldo; void* out2; long long ldo2;
+  float* out_scale; float* out2_scale;   // E4M3 outputs: row scales
 };
 
 constexpr int LN_WARPS = 4;   // rows per block (one warp per row)
 
 // Everything after the x row sits in registers: optional adds, statistics, write-back of the
-// summed row, affine / AdaLN modulation (optionally two modulations), 16-bit stores.
+// summed row, affine / AdaLN modulation (optionally two modulations), 16-bit stores, or
+// (T = E4M3) the row's amax and the E4M3 quantization of the fp32 values.
 // EXACT: D / 4 == 32 * VPL, so the per-vector bounds checks fold away.
 template <typename T, int VPL, bool DUAL, bool EXACT>
 __device__ __forceinline__ void ln_finish(const LnParams& p, const int m, const int lane, float4 (&v)[VPL]) {
@@ -73,8 +76,8 @@ __device__ __forceinline__ void ln_finish(const LnParams& p, const int m, const 
   const float4* sc = p.scale ? reinterpret_cast<const float4*>(p.scale + static_cast<long long>(item) * p.mod_ld) : nullptr;
   const float4* sh2 = p.shift2 ? reinterpret_cast<const float4*>(p.shift2 + static_cast<long long>(item) * p.mod_ld) : nullptr;
   const float4* sc2 = p.scale2 ? reinterpret_cast<const float4*>(p.scale2 + static_cast<long long>(item) * p.mod_ld) : nullptr;
-  uint2* o1 = reinterpret_cast<uint2*>(reinterpret_cast<T*>(p.out) + static_cast<long long>(m) * p.ldo);
-  uint2* o2 = DUAL ? reinterpret_cast<uint2*>(reinterpret_cast<T*>(p.out2) + static_cast<long long>(m) * p.ldo2) : nullptr;
+  T* o1 = reinterpret_cast<T*>(p.out) + static_cast<long long>(m) * p.ldo;
+  T* o2 = DUAL ? reinterpret_cast<T*>(p.out2) + static_cast<long long>(m) * p.ldo2 : nullptr;
   // Each optional vector is applied in its own fully unrolled loop so that its VPL loads
   // are issued back to back (one exposed latency per vector instead of one per element).
 #pragma unroll
@@ -102,13 +105,31 @@ __device__ __forceinline__ void ln_finish(const LnParams& p, const int m, const 
       }
     }
   };
-  auto store_vec = [&](const float4 (&d)[VPL], uint2* dst) {
+  auto store_vec = [&](const float4 (&d)[VPL], T* dst, float* row_scale) {
+    if constexpr (sizeof(T) == 1) {
+      float amax = 0.f;
 #pragma unroll
-    for (int i = 0; i < VPL; ++i) {
-      const int idx = lane + 32 * i;
-      if (idx < nvec) {
-        uint2 pk; pk.x = Cvt<T>::pack2(d[i].x, d[i].y); pk.y = Cvt<T>::pack2(d[i].z, d[i].w);
-        dst[idx] = pk;
+      for (int i = 0; i < VPL; ++i) {
+        const int idx = lane + 32 * i;
+        if (idx < nvec)
+          amax = fmaxf(amax, fmaxf(fmaxf(fabsf(d[i].x), fabsf(d[i].y)), fmaxf(fabsf(d[i].z), fabsf(d[i].w))));
+      }
+      amax = warp_max(amax);
+      const float inv = e4m3_inv(amax);
+#pragma unroll
+      for (int i = 0; i < VPL; ++i) {
+        const int idx = lane + 32 * i;
+        if (idx < nvec) reinterpret_cast<uint32_t*>(dst)[idx] = e4m3x4(d[i].x, d[i].y, d[i].z, d[i].w, inv);
+      }
+      if (lane == 0) row_scale[m] = e4m3_scale(amax);
+    } else {
+#pragma unroll
+      for (int i = 0; i < VPL; ++i) {
+        const int idx = lane + 32 * i;
+        if (idx < nvec) {
+          uint2 pk; pk.x = Cvt<T>::pack2(d[i].x, d[i].y); pk.y = Cvt<T>::pack2(d[i].z, d[i].w);
+          reinterpret_cast<uint2*>(dst)[idx] = pk;
+        }
       }
     }
   };
@@ -120,11 +141,11 @@ __device__ __forceinline__ void ln_finish(const LnParams& p, const int m, const 
     for (int i = 0; i < VPL; ++i) z[i] = v[i];
     if (sc2) mul_vec(z, sc2, 1.f);
     if (sh2) add_vec(z, sh2);
-    store_vec(z, o2);
+    store_vec(z, o2, p.out2_scale);
   }
   if (sc) mul_vec(v, sc, 1.f);
   if (sh) add_vec(v, sh);
-  store_vec(v, o1);
+  store_vec(v, o1, p.out_scale);
 }
 
 template <typename T, int VPL, bool DUAL>
@@ -257,6 +278,51 @@ static int launch_ln2(const LnParams& p, cudaStream_t s) {
 template <typename T>
 static int launch_ln(const LnParams& p, cudaStream_t s) {
   return p.out2 ? launch_ln2<T, true>(p, s) : launch_ln2<T, false>(p, s);
+}
+
+// ------------------------------------------------------------------ E4M3 row quantization
+// One warp per row, 8 elements per lane and step: pass 1 finds the row's amax, pass 2 re-reads
+// the row (from L1 / L2) and writes 8 E4M3 bytes per step.
+constexpr int QR_WARPS = 4;
+
+template <typename T>
+__device__ __forceinline__ void load8(const T* src, float (&v)[8]) {
+  if constexpr (sizeof(T) == 4) {
+    const float4 a = reinterpret_cast<const float4*>(src)[0], b = reinterpret_cast<const float4*>(src)[1];
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+  } else {
+    const uint4 u = *reinterpret_cast<const uint4*>(src);
+    const float2 a = Cvt<T>::unpack2(u.x), b = Cvt<T>::unpack2(u.y), c = Cvt<T>::unpack2(u.z),
+                 d = Cvt<T>::unpack2(u.w);
+    v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y; v[4] = c.x; v[5] = c.y; v[6] = d.x; v[7] = d.y;
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(QR_WARPS * 32) quantize_rows_kernel(const T* __restrict__ x, int M, int K,
+                                                                      long long ld, uint8_t* __restrict__ out,
+                                                                      long long ldo, float* __restrict__ scale) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m = blockIdx.x * QR_WARPS + warp;
+  if (m >= M) return;
+  const T* row = x + static_cast<long long>(m) * ld;
+  const int n8 = K >> 3;
+  float amax = 0.f;
+  for (int c = lane; c < n8; c += 32) {
+    float v[8];
+    load8(row + 8 * c, v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(v[j]));
+  }
+  amax = warp_max(amax);
+  const float inv = e4m3_inv(amax);
+  uint2* orow = reinterpret_cast<uint2*>(out + static_cast<long long>(m) * ldo);
+  for (int c = lane; c < n8; c += 32) {
+    float v[8];
+    load8(row + 8 * c, v);
+    orow[c] = make_uint2(e4m3x4(v[0], v[1], v[2], v[3], inv), e4m3x4(v[4], v[5], v[6], v[7], inv));
+  }
+  if (lane == 0) scale[m] = e4m3_scale(amax);
 }
 
 // ------------------------------------------------------------------ act + cast
@@ -547,11 +613,43 @@ extern "C" int dwm_b200_layernorm(const dwm_layernorm_args* a, dwm_stream_t stre
   p.weight = a->weight; p.bias = a->bias; p.eps = a->eps;
   p.shift = a->shift; p.scale = a->scale; p.shift2 = a->shift2; p.scale2 = a->scale2; p.mod_ld = a->mod_ld;
   p.out = a->out; p.ldo = a->ldo; p.out2 = a->out2; p.ldo2 = a->ldo2;
+  p.out_scale = a->out_scale; p.out2_scale = a->out2_scale;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (a->dtype == DWM_BF16) return launch_ln<__nv_bfloat16>(p, s);
   if (a->dtype == DWM_F16) return launch_ln<__half>(p, s);
-  set_last_error("dwm_b200_layernorm: dtype must be DWM_BF16 or DWM_F16");
+  if (a->dtype == DWM_E4M3) {
+    DWM_REQUIRE(a->out_scale && (!a->out2 || a->out2_scale),
+                "dwm_b200_layernorm: E4M3 output needs out_scale (and out2_scale with out2)");
+    DWM_REQUIRE(!a->out2 || a->ldo2 % 4 == 0, "dwm_b200_layernorm: ldo2 must be a multiple of 4");
+    return launch_ln<__nv_fp8_e4m3>(p, s);
+  }
+  set_last_error("dwm_b200_layernorm: dtype must be DWM_BF16, DWM_F16 or DWM_E4M3");
   return -1;
+}
+
+extern "C" int dwm_b200_quantize_rows(const void* x, int64_t M, int64_t K, int64_t ld, int dtype, void* out,
+                                      int64_t ldo, float* scale, dwm_stream_t stream) {
+  DWM_REQUIRE(x && out && scale, "dwm_b200_quantize_rows: null x/out/scale");
+  DWM_REQUIRE(M > 0 && K > 0 && M < (1ll << 31) && K < (1ll << 31), "dwm_b200_quantize_rows: bad M/K");
+  DWM_REQUIRE(K % 16 == 0 && ld % 8 == 0 && ldo % 16 == 0 && ld >= K && ldo >= K,
+              "dwm_b200_quantize_rows: K and ldo must be multiples of 16 and ld of 8 (ld, ldo >= K); "
+              "got K=%lld ld=%lld ldo=%lld", (long long)K, (long long)ld, (long long)ldo);
+  DWM_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
+              "dwm_b200_quantize_rows: x and out must be 16-byte aligned");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const unsigned grid = static_cast<unsigned>((M + QR_WARPS - 1) / QR_WARPS);
+  const int Mi = static_cast<int>(M), Ki = static_cast<int>(K);
+  uint8_t* o = reinterpret_cast<uint8_t*>(out);
+  if (dtype == DWM_BF16)
+    quantize_rows_kernel<<<grid, QR_WARPS * 32, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(x), Mi, Ki, ld, o, ldo, scale);
+  else if (dtype == DWM_F16)
+    quantize_rows_kernel<<<grid, QR_WARPS * 32, 0, s>>>(reinterpret_cast<const __half*>(x), Mi, Ki, ld, o, ldo, scale);
+  else if (dtype == DWM_F32)
+    quantize_rows_kernel<<<grid, QR_WARPS * 32, 0, s>>>(reinterpret_cast<const float*>(x), Mi, Ki, ld, o, ldo, scale);
+  else
+    DWM_REQUIRE(false, "dwm_b200_quantize_rows: dtype must be DWM_BF16, DWM_F16 or DWM_F32, got %d", dtype);
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
 }
 
 extern "C" int dwm_b200_act_cast(const float* in, void* out, int64_t n, int act, int dtype, dwm_stream_t stream) {

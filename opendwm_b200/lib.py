@@ -9,7 +9,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdwm_b200.so")
 
-DWM_BF16, DWM_F16, DWM_F32 = 0, 1, 2
+DWM_BF16, DWM_F16, DWM_F32, DWM_E4M3 = 0, 1, 2, 3
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU, ACT_RELU = 0, 1, 2, 3, 4
 EPI_STORE, EPI_GEGLU, EPI_QKNORM, EPI_RESID, EPI_F32 = 0, 1, 2, 3, 4
 
@@ -35,6 +35,7 @@ class LinearArgs(ctypes.Structure):
         ("blend_x", _p), ("ldx", _i64),
         ("alpha", _p), ("rows_per_batch", _i64),
         ("peer_out", _p * 8), ("n_peer_out", ctypes.c_int),
+        ("a_scale", _p), ("w_scale", _p), ("out_dtype", ctypes.c_int),
     ]
 
 
@@ -72,6 +73,7 @@ class LayerNormArgs(ctypes.Structure):
         ("mod_ld", _i64),
         ("out", _p), ("ldo", _i64), ("out2", _p), ("ldo2", _i64),
         ("dtype", ctypes.c_int),
+        ("out_scale", _p), ("out2_scale", _p),
     ]
 
 
@@ -99,6 +101,8 @@ SYMBOLS = {
     "dwm_b200_linear": (ctypes.c_int, [ctypes.POINTER(LinearArgs), _p]),
     "dwm_b200_attention": (ctypes.c_int, [ctypes.POINTER(AttentionArgs), _p]),
     "dwm_b200_layernorm": (ctypes.c_int, [ctypes.POINTER(LayerNormArgs), _p]),
+    "dwm_b200_quantize_rows": (ctypes.c_int, [_p, _i64, _i64, _i64, ctypes.c_int, _p, _i64,
+                                              _p, _p]),
     "dwm_b200_act_cast": (ctypes.c_int, [_p, _p, _i64, ctypes.c_int, ctypes.c_int, _p]),
     "dwm_b200_sinusoid": (ctypes.c_int, [_p, _i64, ctypes.c_int, ctypes.c_int,
                                          ctypes.c_float, _p, _i64, ctypes.c_int, _p]),

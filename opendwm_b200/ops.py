@@ -62,12 +62,18 @@ def _rows2d(t, name):
     return t
 
 
+FP8 = torch.float8_e4m3fn
+
+
 def linear(a, w, bias=None, *, epilogue=_l.EPI_STORE, act=_l.ACT_NONE,
            out=None, rows_per_item=0, out_item_stride=0, out_row_offset=0,
            q_norm_weight=None, k_norm_weight=None, qk_region=0, eps=1e-6,
            qk_norm_regions=0, peer_out=None, resid=None, resid_row_mod=0, gate=None, blend_x=None, alpha=None,
-           rows_per_batch=0):
-    """out = epilogue(a @ w.T).  a [M,K], w [N,K] 16-bit; see include/dwm_b200.h."""
+           rows_per_batch=0, a_scale=None, w_scale=None, out_dtype=None):
+    """out = epilogue(a @ w.T).  a [M,K], w [N,K] 16-bit; see include/dwm_b200.h.
+    FP8: a and w float8_e4m3fn with fp32 row scales a_scale [M] and w_scale [N]
+    (quantize_rows / quantize_weight_rows); out_dtype (bf16 / fp16) is the type of the
+    16-bit outputs and is required."""
     _rows2d(a, "a")
     _rows2d(w, "w")
     if not (a.is_cuda and w.is_cuda):
@@ -78,14 +84,31 @@ def linear(a, w, bias=None, *, epilogue=_l.EPI_STORE, act=_l.ACT_NONE,
     N, K2 = w.shape
     if K != K2:
         raise ValueError("K mismatch: a {} vs w {}".format(K, K2))
+    fp8 = a.dtype == FP8
+    if fp8:
+        if a_scale is None or w_scale is None:
+            raise ValueError("FP8 operands need a_scale and w_scale")
+        for t, n, name in ((a_scale, M, "a_scale"), (w_scale, N, "w_scale")):
+            _f32(t, name)
+            if t.dim() != 1 or t.numel() != n:
+                raise ValueError("{} must be fp32 [{}]".format(name, n))
+        if out_dtype not in (torch.bfloat16, torch.float16):
+            raise TypeError("FP8 operands need out_dtype bf16 or fp16, got {}".format(out_dtype))
+        out16 = out_dtype
+    else:
+        if a_scale is not None or w_scale is not None:
+            raise ValueError("a_scale / w_scale go with float8_e4m3fn operands")
+        if out_dtype not in (None, a.dtype):
+            raise TypeError("16-bit operands write their own dtype, not {}".format(out_dtype))
+        out16 = a.dtype
     out_cols = N // 2 if epilogue == _l.EPI_GEGLU else N
     if out is None:
         if epilogue in (_l.EPI_RESID, _l.EPI_F32):
             out = torch.empty((M, out_cols), device=a.device, dtype=torch.float32)
         else:
-            out = torch.empty((M, out_cols), device=a.device, dtype=a.dtype)
+            out = torch.empty((M, out_cols), device=a.device, dtype=out16)
     _rows2d(out, "out")
-    want = torch.float32 if epilogue in (_l.EPI_RESID, _l.EPI_F32) else a.dtype
+    want = torch.float32 if epilogue in (_l.EPI_RESID, _l.EPI_F32) else out16
     if out.dtype != want:
         raise TypeError("out dtype {} != {}".format(out.dtype, want))
     if out.shape[1] < out_cols:
@@ -95,7 +118,11 @@ def linear(a, w, bias=None, *, epilogue=_l.EPI_STORE, act=_l.ACT_NONE,
     args.A, args.lda = a.data_ptr(), a.stride(0)
     args.W, args.ldw = w.data_ptr(), w.stride(0)
     args.bias = _ptr(_f32(bias, "bias"))
-    args.dtype = _dt(a)
+    if fp8:
+        args.dtype, args.out_dtype = _l.DWM_E4M3, _dt(torch.empty(0, dtype=out16))
+        args.a_scale, args.w_scale = a_scale.data_ptr(), w_scale.data_ptr()
+    else:
+        args.dtype = args.out_dtype = _dt(a)
     args.epilogue, args.act = epilogue, act
     args.out, args.ldo = out.data_ptr(), out.stride(0)
     args.rows_per_item = rows_per_item
@@ -136,6 +163,34 @@ def linear(a, w, bias=None, *, epilogue=_l.EPI_STORE, act=_l.ACT_NONE,
         rc = _l.load().dwm_b200_linear(ctypes.byref(args), _stream())
     _l.check(rc, "dwm_b200_linear")
     return out
+
+
+def quantize_rows(x, out=None, scale=None):
+    """Row-wise E4M3 quantization of a bf16 / fp16 / fp32 [M, K] tensor (rows contiguous):
+    returns (out float8_e4m3fn [M, K], scale fp32 [M]) with x[m] ~= out[m] * scale[m];
+    see dwm_b200_quantize_rows for the exact recipe."""
+    _rows2d(x, "x")
+    if not x.is_cuda:
+        raise RuntimeError("dwm_b200 kernels need CUDA tensors (no CPU fallback)")
+    M, K = x.shape
+    if out is None:
+        out = torch.empty(M, K, device=x.device, dtype=FP8)
+    if scale is None:
+        scale = torch.empty(M, device=x.device, dtype=torch.float32)
+    _rows2d(out, "out")
+    _f32(scale, "scale")
+    if out.dtype != FP8 or out.shape[0] != M or out.shape[1] < K or scale.numel() != M:
+        raise ValueError("quantize_rows: out must be float8_e4m3fn [M, >= K], scale fp32 [M]")
+    _l.check(_l.load().dwm_b200_quantize_rows(
+        x.data_ptr(), M, K, x.stride(0), _code(x.dtype), out.data_ptr(), out.stride(0),
+        scale.data_ptr(), _stream()), "dwm_b200_quantize_rows")
+    return out, scale
+
+
+def quantize_weight_rows(w):
+    """nn.Linear weight [N, K] (any float dtype, on the GPU) -> (w8 float8_e4m3fn [N, K],
+    fp32 scale [N]), one scale per output channel, quantized from fp32."""
+    return quantize_rows(w.detach().float().contiguous())
 
 
 def pack_geglu(weight: torch.Tensor, bias=None, block=128):
@@ -219,8 +274,10 @@ def attention(qkv, out, *, D, heads, group_dims, group_strides, seq, inner=None,
 
 def layernorm(x, out, *, weight=None, bias=None, eps=1e-5, add_item=None,
               add_full=None, rows_per_item=0, sum_out=None, shift=None,
-              scale=None, shift2=None, scale2=None, out2=None):
-    """LayerNorm (+adds, +AdaLN modulation) of an fp32 stream into 16-bit out."""
+              scale=None, shift2=None, scale2=None, out2=None, out_scale=None,
+              out2_scale=None):
+    """LayerNorm (+adds, +AdaLN modulation) of an fp32 stream into 16-bit out, or into
+    float8_e4m3fn out (and out2) with fp32 row scales out_scale [M] (out2_scale [M])."""
     _rows2d(_f32(x, "x"), "x")
     _rows2d(out, "out")
     a = _l.LayerNormArgs()
@@ -251,7 +308,18 @@ def layernorm(x, out, *, weight=None, bias=None, eps=1e-5, add_item=None,
     if out2 is not None:
         _rows2d(out2, "out2")
         a.out2, a.ldo2 = out2.data_ptr(), out2.stride(0)
-    a.dtype = _dt(out)
+    if out.dtype == FP8:
+        if out_scale is None or (out2 is not None and (out2_scale is None or out2.dtype != FP8)):
+            raise ValueError("FP8 layernorm output needs out_scale (and an FP8 out2 with out2_scale)")
+        for t, name in ((out_scale, "out_scale"), (out2_scale, "out2_scale")):
+            if t is not None and _f32(t, name).numel() != a.M:
+                raise ValueError("{} must be fp32 [M]".format(name))
+        a.dtype = _l.DWM_E4M3
+        a.out_scale, a.out2_scale = out_scale.data_ptr(), _ptr(out2_scale)
+    else:
+        if out_scale is not None or out2_scale is not None:
+            raise ValueError("out_scale / out2_scale go with a float8_e4m3fn out")
+        a.dtype = _dt(out)
     _l.check(_l.load().dwm_b200_layernorm(ctypes.byref(a), _stream()),
              "dwm_b200_layernorm")
     return out

@@ -31,8 +31,8 @@ from opendwm_b200 import ops as _ops
 from .. import _compat
 from . import adapters as _adapters
 from .crossview_temporal import (
-    AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention,
-    make_feed_forward)
+    AlphaBlender, ParamGroup, VTSelfAttentionBlock, fp8_operand, gemm, make_attention,
+    make_feed_forward, packed)
 
 
 def _sincos_2d(embed_dim, grid_size, base_size, device):
@@ -138,8 +138,15 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         qk_norm_on_additional_modules=None,
         mask_module=None,
         compute_dtype=None,
+        gemm_dtype=None,
     ):
+        """gemm_dtype=torch.float8_e4m3fn runs the linears inside the joint and the
+        cross-view / temporal blocks as E4M3 GEMMs (per-row activation and per-channel weight
+        scales); None keeps every GEMM 16-bit."""
         super().__init__()
+        if gemm_dtype not in (None, torch.float8_e4m3fn):
+            raise ValueError(
+                "gemm_dtype must be None or torch.float8_e4m3fn, got {!r}".format(gemm_dtype))
         if attention_head_dim != 64:
             raise NotImplementedError("kernels are built for head_dim 64")
         if mixer_type != "AlphaBlender":
@@ -171,6 +178,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         self.in_channels = in_channels
         self.out_channels = out_channels
         self.compute_dtype = compute_dtype
+        self.gemm_dtype = gemm_dtype
         self.gradient_checkpointing = False
         self.crossview_gradient_checkpointing = crossview_gradient_checkpointing
         self.temporal_gradient_checkpointing = temporal_gradient_checkpointing
@@ -237,7 +245,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         self.depth_net = None
         self.mask_module = None
 
-        self._pk = None          # packed 16-bit weights
+        self._pk = None          # packed weights (16-bit; E4M3 + scales with gemm_dtype)
         self._ws = {}            # workspaces keyed by shape
         self._cond_key = None
         self._cond = None
@@ -282,7 +290,19 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         def lin(m):
             return w16(m.weight), (None if m.bias is None else f32(m.bias))
 
-        pk = {"dtype": dt}
+        fp8 = self.gemm_dtype is not None
+        pk = {"dtype": dt, "fp8": fp8, "fp8_bytes_saved": 0}
+
+        def blk_lin(w, b):
+            """A linear of a joint block: 16-bit, or E4M3 with per-channel scales."""
+            if not fp8:
+                return w16(w), (None if b is None else f32(b))
+            w8, s = _ops.quantize_weight_rows(w.to(dev))
+            pk["fp8_bytes_saved"] += w.numel() * (dt.itemsize - 1) - 4 * w.shape[0]
+            return w8, (None if b is None else f32(b)), s, dt
+
+        def blin(m):
+            return blk_lin(m.weight, m.bias)
         pe = self.pos_embed.proj
         pk["patch_w"] = w16(pe.weight.reshape(D, -1))
         pk["patch_b"] = f32(pe.bias)
@@ -305,34 +325,34 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
                 b[key] = (off, m.weight.shape[0])
                 off += m.weight.shape[0]
             at = blk.attn
-            b["qkv"] = (w16(torch.cat([at.to_q.weight, at.to_k.weight,
-                                       at.to_v.weight])),
-                        f32(torch.cat([at.to_q.bias, at.to_k.bias, at.to_v.bias])))
-            b["cqkv"] = (w16(torch.cat([at.add_q_proj.weight, at.add_k_proj.weight,
-                                        at.add_v_proj.weight])),
-                         f32(torch.cat([at.add_q_proj.bias, at.add_k_proj.bias,
-                                        at.add_v_proj.bias])))
+            b["qkv"] = blk_lin(torch.cat([at.to_q.weight, at.to_k.weight,
+                                          at.to_v.weight]),
+                               torch.cat([at.to_q.bias, at.to_k.bias, at.to_v.bias]))
+            b["cqkv"] = blk_lin(torch.cat([at.add_q_proj.weight, at.add_k_proj.weight,
+                                           at.add_v_proj.weight]),
+                                torch.cat([at.add_q_proj.bias, at.add_k_proj.bias,
+                                           at.add_v_proj.bias]))
             b["qk_norm"] = at.qk_norm == "rms_norm"
             if b["qk_norm"]:
                 b["nq"], b["nk"] = f32(at.norm_q.weight), f32(at.norm_k.weight)
                 b["ncq"], b["nck"] = f32(at.norm_added_q.weight), \
                     f32(at.norm_added_k.weight)
-            b["out"] = lin(at.to_out[0])
+            b["out"] = blin(at.to_out[0])
             if not blk.context_pre_only:
-                b["cout"] = lin(at.to_add_out)
-                b["cff1"], b["cff2"] = lin(blk.ff_context.net[0].proj), \
-                    lin(blk.ff_context.net[2])
+                b["cout"] = blin(at.to_add_out)
+                b["cff1"], b["cff2"] = blin(blk.ff_context.net[0].proj), \
+                    blin(blk.ff_context.net[2])
             if blk.dual:
                 a2 = blk.attn2
-                b["qkv2"] = (w16(torch.cat([a2.to_q.weight, a2.to_k.weight,
-                                            a2.to_v.weight])),
-                             f32(torch.cat([a2.to_q.bias, a2.to_k.bias,
-                                            a2.to_v.bias])))
+                b["qkv2"] = blk_lin(torch.cat([a2.to_q.weight, a2.to_k.weight,
+                                               a2.to_v.weight]),
+                                    torch.cat([a2.to_q.bias, a2.to_k.bias,
+                                               a2.to_v.bias]))
                 if b["qk_norm"]:
                     b["nq2"], b["nk2"] = f32(a2.norm_q.weight), \
                         f32(a2.norm_k.weight)
-                b["out2"] = lin(a2.to_out[0])
-            b["ff1"], b["ff2"] = lin(blk.ff.net[0].proj), lin(blk.ff.net[2])
+                b["out2"] = blin(a2.to_out[0])
+            b["ff1"], b["ff2"] = blin(blk.ff.net[0].proj), blin(blk.ff.net[2])
             blocks.append(b)
         mod_w.append(self.norm_out.linear.weight.detach())
         mod_b.append(self.norm_out.linear.bias.detach())
@@ -347,13 +367,15 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
             pk["ve1"], pk["ve2"] = lin(self.view_embedding.linear_1), \
                 lin(self.view_embedding.linear_2)
         if self.enable_crossview:
-            pk["cv"] = [b.pack(dt, dev) for b in self.crossview_transformer_blocks]
+            pk["cv"] = [b.pack(dt, dev, fp8) for b in self.crossview_transformer_blocks]
             pk["vpe"] = [(lin(m.linear_1), lin(m.linear_2))
                          for m in self.view_pos_embeds]
         if self.enable_temporal:
-            pk["tp"] = [b.pack(dt, dev) for b in self.temporal_transformer_blocks]
+            pk["tp"] = [b.pack(dt, dev, fp8) for b in self.temporal_transformer_blocks]
             pk["tpe"] = [(lin(m.linear_1), lin(m.linear_2))
                          for m in self.time_pos_embeds]
+        # weight bytes the E4M3 copies save against 16-bit ones (scales included)
+        pk["fp8_bytes_saved"] += sum(p["fp8_bytes_saved"] for p in pk.get("cv", []) + pk.get("tp", []))
         self._pk = pk
         return pk
 
@@ -384,6 +406,14 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
             "tokens": e(N * S, self.patch_size ** 2 * self.out_channels,
                         dtype=torch.float32),
         }
+        if pk["fp8"]:
+            # E4M3 operands + row scales: LayerNorm outputs (a8*, ac8) and the quantized
+            # 16-bit GEMM outputs (q8 sample rows, qc8 context rows)
+            f8 = torch.float8_e4m3fn
+            for k, rows, cols in (("a8", N * S, D), ("a8b", N * S, D), ("ac8", N * L, D),
+                                  ("q8", N * S, 4 * D), ("qc8", N * L, 4 * D)):
+                ws[k] = e(rows, cols, dtype=f8)
+                ws[k + "_s"] = e(rows, dtype=torch.float32)
         self._ws = {key: ws}  # keep a single live workspace
         return ws
 
@@ -625,13 +655,13 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         remap = dict(rows_per_item=T_loc * V * S, out_item_stride=T * V * S,
                      out_row_offset=plan.t_offset * V * S)
 
-        def project(p, a16, w, b, nw, out, peer_out=None, **kw):
+        def project(p, a16, w, nw, out, peer_out=None, **kw):
             if p["qk_norm"]:
-                _ops.linear(a16, w, b, epilogue=_lib.EPI_QKNORM, out=out,
-                            q_norm_weight=nw, qk_region=D, qk_norm_regions=1,
-                            eps=eps, peer_out=peer_out, **kw)
+                gemm(a16, w, epilogue=_lib.EPI_QKNORM, out=out,
+                     q_norm_weight=nw, qk_region=D, qk_norm_regions=1,
+                     eps=eps, peer_out=peer_out, **kw)
             else:
-                _ops.linear(a16, w, b, out=out, peer_out=peer_out, **kw)
+                gemm(a16, w, out=out, peer_out=peer_out, **kw)
 
         def attend(kv_all, out):
             if kind == "full":         # (b v) (t hw)
@@ -661,14 +691,14 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
                 # fused: the K,V GEMM epilogue scatters its tiles into every peer's
                 # gathered buffer over NVLink; one group barrier publishes them
                 kv_all, peers, hdl = peer_kv.next()
-                project(p, a16, p["kv_w"], p["kv_b"], p.get("nk"), kv_all, peers, **remap)
-                project(p, a16, p["q_w"], p["q_b"], p.get("nq"), q_loc)
+                project(p, a16, packed(p, "kv"), p.get("nk"), kv_all, peers, **remap)
+                project(p, a16, packed(p, "q"), p.get("nq"), q_loc)
                 hdl.barrier(channel=0)
             else:
                 kv_loc, kv_all = ws["kv_loc"], ws["kv_all"]
-                project(p, a16, p["kv_w"], p["kv_b"], p.get("nk"), kv_loc)
+                project(p, a16, packed(p, "kv"), p.get("nk"), kv_loc)
                 work = plan.gather_frames_kv(kv_loc, kv_all, batch=B, async_op=True)
-                project(p, a16, p["q_w"], p["q_b"], p.get("nq"), q_loc)
+                project(p, a16, packed(p, "q"), p.get("nq"), q_loc)
                 work.wait()
             attend(kv_all, out)
         return qkv_attend
@@ -679,8 +709,23 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         x, c, mod = ws["x"], ws["c"], ws["mod"]
         c_src = ws.pop("c_in", None)          # first block: context read from the cache
         c_src = c if c_src is None else c_src
-        a16, a16b, ac16 = ws["a16"], ws["a16b"], ws["ac16"]
         qkv, o16, oc16 = ws["qkv_j"], ws["o16"], ws["oc16"]
+        fp8 = self._pk["fp8"]
+        if fp8:   # LayerNorms write E4M3 operands with row scales
+            a16, a16b, ac16 = [(ws[k], ws[k + "_s"]) for k in ("a8", "a8b", "ac8")]
+        else:
+            a16, a16b, ac16 = ws["a16"], ws["a16b"], ws["ac16"]
+
+        def ln(src, dst, **kw):
+            if fp8:
+                if "out2" in kw:
+                    kw["out2"], kw["out2_scale"] = kw["out2"]
+                _ops.layernorm(src, dst[0], out_scale=dst[1], **kw)
+            else:
+                _ops.layernorm(src, dst, **kw)
+
+        def operand(t, key):    # the 16-bit GEMM output t as the next GEMM's operand
+            return fp8_operand(ws, key, t) if fp8 else t
         o, _ = b["mod"]
         m = [mod[:, o + i * D:o + (i + 1) * D] for i in range(9 if b["dual"] else 6)]
         shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp = m[:6]
@@ -696,55 +741,51 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
             kw = dict(shift2=m[6], scale2=m[7], out2=a16b)
         if residual is not None:   # hidden_states += condition residual (:491-494)
             kw.update(add_full=residual, sum_out=x)
-        _ops.layernorm(x, a16, eps=1e-6, rows_per_item=S, shift=shift_msa,
-                       scale=scale_msa, **kw)
-        _ops.layernorm(c_src, ac16, eps=1e-6, rows_per_item=L, shift=c_shift_msa,
-                       scale=c_scale_msa)
+        ln(x, a16, eps=1e-6, rows_per_item=S, shift=shift_msa, scale=scale_msa, **kw)
+        ln(c_src, ac16, eps=1e-6, rows_per_item=L, shift=c_shift_msa, scale=c_scale_msa)
         if b["qk_norm"]:
-            _ops.linear(a16, *b["qkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
-                        rows_per_item=S, out_item_stride=S + L, out_row_offset=0,
-                        q_norm_weight=b["nq"], k_norm_weight=b["nk"], qk_region=D,
-                        eps=1e-6)
-            _ops.linear(ac16, *b["cqkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
-                        rows_per_item=L, out_item_stride=S + L, out_row_offset=S,
-                        q_norm_weight=b["ncq"], k_norm_weight=b["nck"],
-                        qk_region=D, eps=1e-6)
+            gemm(a16, b["qkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
+                 rows_per_item=S, out_item_stride=S + L, out_row_offset=0,
+                 q_norm_weight=b["nq"], k_norm_weight=b["nk"], qk_region=D,
+                 eps=1e-6)
+            gemm(ac16, b["cqkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
+                 rows_per_item=L, out_item_stride=S + L, out_row_offset=S,
+                 q_norm_weight=b["ncq"], k_norm_weight=b["nck"],
+                 qk_region=D, eps=1e-6)
         else:
-            _ops.linear(a16, *b["qkv"], out=qkv, rows_per_item=S,
-                        out_item_stride=S + L, out_row_offset=0)
-            _ops.linear(ac16, *b["cqkv"], out=qkv, rows_per_item=L,
-                        out_item_stride=S + L, out_row_offset=S)
+            gemm(a16, b["qkv"], out=qkv, rows_per_item=S,
+                 out_item_stride=S + L, out_row_offset=0)
+            gemm(ac16, b["cqkv"], out=qkv, rows_per_item=L,
+                 out_item_stride=S + L, out_row_offset=S)
         # joint attention over [sample ; context] tokens of each view-frame
         _ops.attention(qkv, o16, D=D, heads=heads, group_dims=[N],
                        group_strides=[S + L], seq=S + L, out_group_strides=[S],
                        out_stride_outer=0, out_stride_inner=1, split=S, out2=oc16)
-        _ops.linear(o16, *b["out"], epilogue=_lib.EPI_RESID, resid=x, out=x,
-                    gate=gate_msa, rows_per_item=S)
+        gemm(operand(o16, "q8"), b["out"], epilogue=_lib.EPI_RESID, resid=x, out=x,
+             gate=gate_msa, rows_per_item=S)
         if b["dual"]:
             q2 = ws["qkv_s"]
             if b["qk_norm"]:
-                _ops.linear(a16b, *b["qkv2"], epilogue=_lib.EPI_QKNORM, out=q2,
-                            q_norm_weight=b["nq2"], k_norm_weight=b["nk2"],
-                            qk_region=D, eps=1e-6)
+                gemm(a16b, b["qkv2"], epilogue=_lib.EPI_QKNORM, out=q2,
+                     q_norm_weight=b["nq2"], k_norm_weight=b["nk2"],
+                     qk_region=D, eps=1e-6)
             else:
-                _ops.linear(a16b, *b["qkv2"], out=q2)
+                gemm(a16b, b["qkv2"], out=q2)
             _ops.attention(q2, o16, D=D, heads=heads, group_dims=[N],
                            group_strides=[S], seq=S)
-            _ops.linear(o16, *b["out2"], epilogue=_lib.EPI_RESID, resid=x, out=x,
-                        gate=m[8], rows_per_item=S)
-        _ops.layernorm(x, a16, eps=1e-6, rows_per_item=S, shift=shift_mlp,
-                       scale=scale_mlp)
-        _ops.linear(a16, *b["ff1"], act=_lib.ACT_GELU_TANH, out=ws["g16"])
-        _ops.linear(ws["g16"], *b["ff2"], epilogue=_lib.EPI_RESID, resid=x, out=x,
-                    gate=gate_mlp, rows_per_item=S)
+            gemm(operand(o16, "q8"), b["out2"], epilogue=_lib.EPI_RESID, resid=x, out=x,
+                 gate=m[8], rows_per_item=S)
+        ln(x, a16, eps=1e-6, rows_per_item=S, shift=shift_mlp, scale=scale_mlp)
+        gemm(a16, b["ff1"], act=_lib.ACT_GELU_TANH, out=ws["g16"])
+        gemm(operand(ws["g16"], "q8"), b["ff2"], epilogue=_lib.EPI_RESID, resid=x, out=x,
+             gate=gate_mlp, rows_per_item=S)
         if not b["last"]:
-            _ops.linear(oc16, *b["cout"], epilogue=_lib.EPI_RESID, resid=c_src, out=c,
-                        gate=c_gate_msa, rows_per_item=L)
-            _ops.layernorm(c, ac16, eps=1e-6, rows_per_item=L, shift=c_shift_mlp,
-                           scale=c_scale_mlp)
-            _ops.linear(ac16, *b["cff1"], act=_lib.ACT_GELU_TANH, out=ws["gc16"])
-            _ops.linear(ws["gc16"], *b["cff2"], epilogue=_lib.EPI_RESID, resid=c,
-                        out=c, gate=c_gate_mlp, rows_per_item=L)
+            gemm(operand(oc16, "qc8"), b["cout"], epilogue=_lib.EPI_RESID, resid=c_src,
+                 out=c, gate=c_gate_msa, rows_per_item=L)
+            ln(c, ac16, eps=1e-6, rows_per_item=L, shift=c_shift_mlp, scale=c_scale_mlp)
+            gemm(ac16, b["cff1"], act=_lib.ACT_GELU_TANH, out=ws["gc16"])
+            gemm(operand(ws["gc16"], "qc8"), b["cff2"], epilogue=_lib.EPI_RESID, resid=c,
+                 out=c, gate=c_gate_mlp, rows_per_item=L)
 
     # -- forward -------------------------------------------------------------------------------
     @torch.no_grad()
