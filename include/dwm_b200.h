@@ -283,7 +283,8 @@ int dwm_b200_euler_step_by_indices(const float* model_output, float* sample, int
  *   out    rows = nb*(tp-kt+1)*h*w pixels, c_out columns (channels-last), pitch ldo
  * spatial zero padding kh/2, kw/2; no implicit temporal padding.  c_out must be a multiple
  * of 32 (pad the weight rows); tiles of 256 / 128 / 64 / 32 output channels.  Epilogues: DWM_EPI_STORE (16-bit,
- * bias + act), DWM_EPI_F32, DWM_EPI_RESID (fp32: acc + bias + resid).
+ * bias + act), DWM_EPI_F32, DWM_EPI_RESID (fp32: acc + bias + resid).  Opt-in E4M3 x and
+ * weight with per-volume / per-channel scales (a_scale, w_scale below), RESID only.
  * Replaces diffusers CogVideoXCausalConv3d / CogVideoXUpsample3D.conv inside
  * AutoencoderKLCogVideoX.decode (called at ctsd.py:1634-1640, 1615-1617) and the
  * AdapterResnetBlock 3x3 convs (adapters.py:20). */
@@ -311,6 +312,14 @@ typedef struct dwm_conv_args {
   int64_t ldx;
   const float* alpha;
   int64_t rows_per_batch;
+  /* FP8 (dtype == DWM_E4M3; epilogue DWM_EPI_RESID only): x and weight are E4M3, with
+   * a_scale fp32 [nb] (one scale per VOLUME: every tap of an output pixel reads the same
+   * volume) and w_scale fp32 [c_out] (one per output channel, over all taps and input
+   * channels; 8-byte aligned).  The fp32 accumulator is multiplied by a_scale[nb] *
+   * w_scale[n] before the bias / residual / blend.  c_in must be a multiple of 16; a ragged
+   * last 128-channel block is zero-filled.  Channel blocks are 128 E4M3 elements. */
+  const float* a_scale;
+  const float* w_scale;
 } dwm_conv_args;
 
 int dwm_b200_conv(const dwm_conv_args* args, dwm_stream_t stream);
@@ -336,6 +345,18 @@ int dwm_b200_spatialnorm_silu(const float* x, int64_t nb, int64_t T, int64_t H, 
                               const float* beta, const float* zy, const float* zb, int Tz, int hz,
                               int wz, int apply_silu, void* out, int64_t out_T, int64_t out_t0,
                               int dtype, dwm_stream_t stream);
+/* GroupNorm(+SiLU) with an E4M3 output, the operand of an FP8 dwm_b200_conv: the values of
+ * dwm_b200_spatialnorm_silu with zy = zb = NULL (the fp32 y the 16-bit path would round),
+ * quantized with ONE scale per volume n: amax = max |y| over the volume's T frames;
+ * amax == 0 -> out_scale[n] = 1, q = 0; otherwise q = cvt.rn.satfinite.e4m3(y * (448 / amax)),
+ * out_scale[n] = amax / 448 (IEEE fp32).  out is E4M3 [nb, out_T, H, W, C]; only frames
+ * [out_t0, out_t0 + T) are written (the leading cache frames stay as they are).  Two passes
+ * over x (amax, then quantize); out_scale (fp32 [nb]) is the amax scratch in between, so the
+ * call allocates nothing.  C must be a multiple of 16. */
+int dwm_b200_groupnorm_silu_e4m3(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C,
+                                 int groups, const double* sums, float eps, const float* gamma,
+                                 const float* beta, int apply_silu, void* out, int64_t out_T,
+                                 int64_t out_t0, float* out_scale, dwm_stream_t stream);
 /* CogVideoXUpsample3D interpolation: nearest x2 in H, W and (compress_time) in T, where an
  * odd T > 1 keeps its first frame un-doubled in time; fp32 in, 16-bit out
  * [nb, T', 2H, 2W, C].  Also the F.interpolate(nearest, x2) of the UNet / AutoencoderKL

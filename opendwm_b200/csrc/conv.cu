@@ -7,14 +7,23 @@
 // caller provides TP = T_out + KT - 1 frames (causal convolutions keep their cache /
 // replicated frames in front).
 //
-// Used by: CogVideoX causal conv3d (3x3x3), its per-frame upsampler conv2d (1x3x3), and
-// the T2I-adapter 3x3 convs.  Epilogues are the GEMM ones (bias/act store, fp32 residual).
+// Used by: CogVideoX causal conv3d (3x3x3), its per-frame upsampler conv2d (1x3x3), the
+// T2I-adapter 3x3 convs and the UNet ResBlock convs.  Epilogues are the GEMM ones (bias/act
+// store, fp32 residual).
+//
+// FP8 (opt-in, RESID epilogue only): E4M3 activations with ONE fp32 scale per volume nb and
+// E4M3 weights with one scale per output channel (over all taps and input channels).  A
+// per-pixel scale could not be factored out of a sum over taps that read different pixels;
+// a volume scale can, because tiles never cross volumes and the padding is zero.  A stage is
+// still 128 bytes of K per pixel row (128 E4M3 channels, four k32 MMAs), so the patch, halo
+// and weight-slice layouts and every descriptor step are the 16-bit ones.
 #include "gemm_epilogue.cuh"
 
 namespace dwm {
 
 constexpr int CV_STAGES = 4;
-constexpr int CV_A_BYTES = 128 * BK * 2;
+constexpr int CV_ROW_BYTES = BK * 2;           // bytes of K per pixel row and stage (either precision)
+constexpr int CV_A_BYTES = 128 * CV_ROW_BYTES;
 
 struct ConvGeom {
   int nb, t_out, h, w;
@@ -47,12 +56,14 @@ struct ConvCfg {
   static constexpr int kSmemBytes = kStages * (kABytes + kBBytes) + EPI_STAGE_BYTES + 1024 + 256;
 };
 
-template <typename T, int EPI, int CBN, int CL, bool HALO>
+// TA: operand type (bf16 / fp16 / E4M3); T: type of the 16-bit outputs (TA unless E4M3)
+template <typename TA, typename T, int EPI, int CBN, int CL, bool HALO>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                       const ConvGeom g, EpiParams p) {
   using Cfg = ConvCfg<CBN, HALO>;
   constexpr int A_BYTES = Cfg::kABytes, B_BYTES = Cfg::kBBytes, STAGES = Cfg::kStages;
+  constexpr int BKE = CV_ROW_BYTES / static_cast<int>(sizeof(TA));   // channels per stage
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
@@ -65,15 +76,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
   const int n_blocks = (g.c_out + CBN - 1) / CBN;
-  const int c_blocks = (g.c_in + BK - 1) / BK;
+  const int c_blocks = (g.c_in + BKE - 1) / BKE;   // a ragged last block is TMA zero fill
   const int outer_taps = HALO ? g.kt * g.kh : g.kt * g.kh * g.kw;   // HALO: dw runs inside the stage
   const int k_iters = outer_taps * c_blocks;
   const int w_tiles = HALO ? (g.w + 127) / 128 : g.tiles_w;
   const long long m_tiles = static_cast<long long>(g.nb) * g.t_out * (HALO ? g.h * w_tiles : g.tiles_w * g.tiles_h);
   const long long num_tiles = ((m_tiles + CL - 1) / CL) * n_blocks;
   const long long first = static_cast<long long>(blockIdx.x) / CL, step = static_cast<long long>(gridDim.x) / CL;
-  const uint32_t stage_tx = HALO ? static_cast<uint32_t>(CVH_A_ROWS * BK * 2 + B_BYTES)
-                                 : static_cast<uint32_t>(g.bw * g.bh * BK * 2 + B_BYTES);
+  const uint32_t stage_tx = HALO ? static_cast<uint32_t>(CVH_A_ROWS * CV_ROW_BYTES + B_BYTES)
+                                 : static_cast<uint32_t>(g.bw * g.bh * CV_ROW_BYTES + B_BYTES);
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_x);
@@ -118,20 +129,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             mbar_expect_tx(&full_bar[stage], stage_tx);
             uint8_t* sb = smem_b + stage * B_BYTES;
             if constexpr (HALO) {
-              tma_load_5d(&tmap_x, &full_bar[stage], smem_a + stage * A_BYTES, cb * BK, w0 - 1,
+              tma_load_5d(&tmap_x, &full_bar[stage], smem_a + stage * A_BYTES, cb * BKE, w0 - 1,
                           h0 + dh - g.kh / 2, t + dt, nb, kEvictNormal);
 #pragma unroll
               for (int d = 0; d < 3; ++d)
-                tma_load_2d(&tmap_w, &full_bar[stage], sb + d * CBN * BK * 2, cb * BK,
+                tma_load_2d(&tmap_w, &full_bar[stage], sb + d * CBN * CV_ROW_BYTES, cb * BKE,
                             (ot * 3 + d) * g.c_out + n_blk * CBN, kEvictLast);
             } else {
-              tma_load_5d(&tmap_x, &full_bar[stage], smem_a + stage * A_BYTES, cb * BK,
+              tma_load_5d(&tmap_x, &full_bar[stage], smem_a + stage * A_BYTES, cb * BKE,
                           w0 + dw - g.kw / 2, h0 + dh - g.kh / 2, t + dt, nb, kEvictNormal);
               if constexpr (CL == 2)
-                tma_load_2d_mc(&tmap_w, &full_bar[stage], sb + rank * (B_BYTES / 2), cb * BK,
+                tma_load_2d_mc(&tmap_w, &full_bar[stage], sb + rank * (B_BYTES / 2), cb * BKE,
                                ot * g.c_out + n_blk * CBN + static_cast<int>(rank) * (CBN / 2), 0x3, kEvictLast);
               else
-                tma_load_2d(&tmap_w, &full_bar[stage], sb, cb * BK, ot * g.c_out + n_blk * CBN, kEvictLast);
+                tma_load_2d(&tmap_w, &full_bar[stage], sb, cb * BKE, ot * g.c_out + n_blk * CBN, kEvictLast);
             }
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
@@ -150,9 +161,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       int n_blk, w0, h0, t, nb;
       const bool valid = decode(tile, n_blk, w0, h0, t, nb);
       float acc[CBN / 2];
-      wg_mainloop<T, CBN, CL, Cfg::kTaps>(acc, smem_a, A_BYTES, cw * 64 * 128, smem_b, B_BYTES, full_bar, empty_bar,
+      wg_mainloop<TA, CBN, CL, Cfg::kTaps>(acc, smem_a, A_BYTES, cw * 64 * 128, smem_b, B_BYTES, full_bar, empty_bar,
                                           STAGES, k_iters, stage, phase, lane, rank ^ 1u);
-      if (!valid) continue;
+      if (!valid) continue;   // (the dummy tile's nb == g.nb has no scale)
+      if constexpr (sizeof(TA) == 1) dequant_frag_vol<CBN>(acc, __ldg(p.a_scale + nb), p.w_scale, n_blk * CBN, g.c_out, lane);
       TileGeom tg;
       tg.bw = HALO ? 128 : g.bw; tg.rows = HALO ? 128 : g.bw * g.bh;
       tg.w_lim = g.w - w0; tg.h_lim = HALO ? 1 : g.h - h0; tg.img_w = g.w;
@@ -168,8 +180,10 @@ int make_tmap_nd(CUtensorMap* map, const void* base, int rank, const uint64_t* d
 
 extern int g_conv_2cta, g_conv_halo;
 
-template <typename T, int EPI, int CBN>
+template <typename TA, typename T, int EPI, int CBN>
 static int launch_conv(const dwm_conv_args* a, cudaStream_t stream) {
+  constexpr int eb = static_cast<int>(sizeof(TA));
+  constexpr uint32_t BKE = CV_ROW_BYTES / eb;
   ConvGeom g;
   g.nb = static_cast<int>(a->nb);
   g.kt = a->kt; g.kh = a->kh; g.kw = a->kw;
@@ -186,14 +200,14 @@ static int launch_conv(const dwm_conv_args* a, cudaStream_t stream) {
   CUtensorMap tx, tw;
   const uint64_t dims[5] = {static_cast<uint64_t>(a->c_in), static_cast<uint64_t>(a->w), static_cast<uint64_t>(a->h),
                             static_cast<uint64_t>(a->tp), static_cast<uint64_t>(a->nb)};
-  const uint64_t st[4] = {static_cast<uint64_t>(a->c_in) * 2, static_cast<uint64_t>(a->c_in) * a->w * 2,
-                          static_cast<uint64_t>(a->c_in) * a->w * a->h * 2,
-                          static_cast<uint64_t>(a->c_in) * a->w * a->h * a->tp * 2};
-  const uint32_t box[5] = {BK, static_cast<uint32_t>(g.bw), static_cast<uint32_t>(g.bh), 1, 1};
-  int rc = make_tmap_nd(&tx, a->x, 5, dims, st, box, 2);
+  const uint64_t st[4] = {static_cast<uint64_t>(a->c_in) * eb, static_cast<uint64_t>(a->c_in) * a->w * eb,
+                          static_cast<uint64_t>(a->c_in) * a->w * a->h * eb,
+                          static_cast<uint64_t>(a->c_in) * a->w * a->h * a->tp * eb};
+  const uint32_t box[5] = {BKE, static_cast<uint32_t>(g.bw), static_cast<uint32_t>(g.bh), 1, 1};
+  int rc = make_tmap_nd(&tx, a->x, 5, dims, st, box, eb);
   if (rc) return rc;
   const int taps = a->kt * a->kh * a->kw;
-  rc = make_tmap_2d(&tw, a->weight, static_cast<uint64_t>(taps) * a->c_out, a->c_in, a->c_in, CBN, BK, 2);
+  rc = make_tmap_2d(&tw, a->weight, static_cast<uint64_t>(taps) * a->c_out, a->c_in, a->c_in, CBN, BKE, eb);
   if (rc) return rc;
 
   EpiParams p = {};
@@ -204,6 +218,8 @@ static int launch_conv(const dwm_conv_args* a, cudaStream_t stream) {
   p.blend_x = a->blend_x; p.ldx = a->ldx; p.alpha = a->alpha; p.rows_per_batch = a->rows_per_batch;
   p.norm_regions = 2;
   p.n_peers = 0;
+  p.a_scale = a->a_scale;
+  p.w_scale = a->w_scale;
 
   const long long n_blocks = (g.c_out + CBN - 1) / CBN;
   const long long m_tiles = static_cast<long long>(g.nb) * g.t_out * g.tiles_w * g.tiles_h;
@@ -238,33 +254,33 @@ static int launch_conv(const dwm_conv_args* a, cudaStream_t stream) {
     // (C_out tiles of 256 columns: three weight slices per stage would not fit)
     if (g_conv_halo == 1 && a->kw == 3 && g.w >= 128 && seg_tiles * n_blocks >= sms) {
       CUtensorMap txh;
-      const uint32_t boxh[5] = {BK, static_cast<uint32_t>(CVH_A_ROWS), 1, 1, 1};
-      rc = make_tmap_nd(&txh, a->x, 5, dims, st, boxh, 2);
+      const uint32_t boxh[5] = {BKE, static_cast<uint32_t>(CVH_A_ROWS), 1, 1, 1};
+      rc = make_tmap_nd(&txh, a->x, 5, dims, st, boxh, eb);
       if (rc) return rc;
-      return go(conv_wgmma_kernel<T, EPI, CBN, 1, true>, attr_halo, ConvCfg<CBN, true>::kSmemBytes, 1, seg_tiles, txh, tw);
+      return go(conv_wgmma_kernel<TA, T, EPI, CBN, 1, true>, attr_halo, ConvCfg<CBN, true>::kSmemBytes, 1, seg_tiles, txh, tw);
     }
   }
   if constexpr (CBN >= 64) {
     // pairs once there are enough pixel tiles for both CTAs of every cluster (the weight half
     // of a CTA must be whole 8-row swizzle atoms)
     if (g_conv_2cta == 1 && m_tiles * n_blocks >= 2 * sms) {
-      rc = make_tmap_2d(&tw, a->weight, static_cast<uint64_t>(taps) * a->c_out, a->c_in, a->c_in, CBN / 2, BK, 2);
+      rc = make_tmap_2d(&tw, a->weight, static_cast<uint64_t>(taps) * a->c_out, a->c_in, a->c_in, CBN / 2, BKE, eb);
       if (rc) return rc;
-      return go(conv_wgmma_kernel<T, EPI, CBN, 2, false>, attr_pair, ConvCfg<CBN, false>::kSmemBytes, 2, m_tiles, tx, tw);
+      return go(conv_wgmma_kernel<TA, T, EPI, CBN, 2, false>, attr_pair, ConvCfg<CBN, false>::kSmemBytes, 2, m_tiles, tx, tw);
     }
   }
-  return go(conv_wgmma_kernel<T, EPI, CBN, 1, false>, attr_one, ConvCfg<CBN, false>::kSmemBytes, 1, m_tiles, tx, tw);
+  return go(conv_wgmma_kernel<TA, T, EPI, CBN, 1, false>, attr_one, ConvCfg<CBN, false>::kSmemBytes, 1, m_tiles, tx, tw);
 }
 
 int g_conv_2cta = -1;   // -1: env DWM_CONV_2CTA (default 1); option "conv_2cta"
 int g_conv_halo = -1;   // -1: env DWM_CONV_HALO (default 1); option "conv_halo"
 
-template <typename T, int EPI>
+template <typename TA, typename T, int EPI>
 static int conv_pick_bn(const dwm_conv_args* a, cudaStream_t s) {
-  if (a->c_out % 256 == 0) return launch_conv<T, EPI, 256>(a, s);
-  if (a->c_out % 128 == 0) return launch_conv<T, EPI, 128>(a, s);
-  if (a->c_out % 64 == 0) return launch_conv<T, EPI, 64>(a, s);
-  if (a->c_out % 32 == 0) return launch_conv<T, EPI, 32>(a, s);
+  if (a->c_out % 256 == 0) return launch_conv<TA, T, EPI, 256>(a, s);
+  if (a->c_out % 128 == 0) return launch_conv<TA, T, EPI, 128>(a, s);
+  if (a->c_out % 64 == 0) return launch_conv<TA, T, EPI, 64>(a, s);
+  if (a->c_out % 32 == 0) return launch_conv<TA, T, EPI, 32>(a, s);
   set_last_error("dwm_b200_conv: C_out must be a multiple of 32 (pad the weight rows); got %lld", (long long)a->c_out);
   return -1;
 }
@@ -272,9 +288,9 @@ static int conv_pick_bn(const dwm_conv_args* a, cudaStream_t s) {
 template <typename T>
 static int conv_pick_epi(const dwm_conv_args* a, cudaStream_t s) {
   switch (a->epilogue) {
-    case DWM_EPI_STORE: return conv_pick_bn<T, DWM_EPI_STORE>(a, s);
-    case DWM_EPI_RESID: return conv_pick_bn<T, DWM_EPI_RESID>(a, s);
-    case DWM_EPI_F32: return conv_pick_bn<T, DWM_EPI_F32>(a, s);
+    case DWM_EPI_STORE: return conv_pick_bn<T, T, DWM_EPI_STORE>(a, s);
+    case DWM_EPI_RESID: return conv_pick_bn<T, T, DWM_EPI_RESID>(a, s);
+    case DWM_EPI_F32: return conv_pick_bn<T, T, DWM_EPI_F32>(a, s);
     default: set_last_error("dwm_b200_conv: epilogue must be STORE, RESID or F32"); return -1;
   }
 }
@@ -297,6 +313,16 @@ extern "C" int dwm_b200_conv(const dwm_conv_args* a, dwm_stream_t stream) {
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (a->dtype == DWM_BF16) return conv_pick_epi<__nv_bfloat16>(a, s);
   if (a->dtype == DWM_F16) return conv_pick_epi<__half>(a, s);
-  set_last_error("dwm_b200_conv: dtype must be DWM_BF16 or DWM_F16");
+  if (a->dtype == DWM_E4M3) {
+    DWM_REQUIRE(a->epilogue == DWM_EPI_RESID, "dwm_b200_conv: E4M3 operands need epilogue DWM_EPI_RESID, got %d",
+                a->epilogue);
+    DWM_REQUIRE(a->a_scale && a->w_scale, "dwm_b200_conv: E4M3 operands need a_scale [nb] and w_scale [c_out]");
+    DWM_REQUIRE(a->c_in % 16 == 0, "dwm_b200_conv: E4M3 needs C_in %% 16 == 0 (16-byte TMA pitch); got %lld",
+                (long long)a->c_in);
+    DWM_REQUIRE((reinterpret_cast<uintptr_t>(a->w_scale) & 7) == 0, "dwm_b200_conv: w_scale must be 8-byte aligned");
+    // the fp32-output epilogue never names its 16-bit type
+    return conv_pick_bn<__nv_fp8_e4m3, __nv_bfloat16, DWM_EPI_RESID>(a, s);
+  }
+  set_last_error("dwm_b200_conv: dtype must be DWM_BF16, DWM_F16 or DWM_E4M3");
   return -1;
 }

@@ -360,6 +360,34 @@ __device__ __forceinline__ void dequant_frag(float (&acc)[NT / 2], const float* 
   }
 }
 
+// FP8 convolution: acc[r, n] *= s * w_scale[n], where s is the activation scale of the tile's
+// volume (every tap of an output pixel reads its own volume, so one scalar covers the tile).
+// Same rounding as dequant_frag: the scale product is rounded once, then one rounded multiply.
+template <int NT>
+__device__ __forceinline__ void dequant_frag_vol(float (&acc)[NT / 2], float s, const float* w_scale,
+                                                 int n_tile0, int N, int lane) {
+#pragma unroll
+  for (int g = 0; g < NT / 32; ++g) {
+    constexpr int G = 4;   // n8 blocks per group (a 32-column chunk)
+    float2 w[G];
+#pragma unroll
+    for (int jj = 0; jj < G; ++jj) {
+      const int col = n_tile0 + 8 * (G * g + jj) + 2 * (lane & 3);
+      w[jj] = col < N ? __ldg(reinterpret_cast<const float2*>(w_scale + col)) : make_float2(0.f, 0.f);
+    }
+#pragma unroll
+    for (int jj = 0; jj < G; ++jj) {
+      const int j = G * g + jj;
+      const float sx = __fmul_rn(s, w[jj].x), sy = __fmul_rn(s, w[jj].y);
+      acc[4 * j + 0] = __fmul_rn(acc[4 * j + 0], sx);
+      acc[4 * j + 1] = __fmul_rn(acc[4 * j + 1], sy);
+      acc[4 * j + 2] = __fmul_rn(acc[4 * j + 2], sx);
+      acc[4 * j + 3] = __fmul_rn(acc[4 * j + 3], sy);
+    }
+    asm volatile("" ::: "memory");
+  }
+}
+
 // One output tile of one consumer warpgroup: acc[64 x NT] = sum over k_iters stages and TAPS
 // taps of A[64 rows at a_row_off (+ t rows for tap t)] . B[NT rows of tap t]^T.  TAPS = 3 is
 // the halo-row convolution: the three dw taps read row-shifted views of one A tile.  Every stage

@@ -130,7 +130,9 @@ int make_tmap_nd(CUtensorMap* map, const void* base, int rank, const uint64_t* d
   cuuint32_t bx[5], estr[5];
   for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bx[i] = box[i]; estr[i] = 1; }
   for (int i = 0; i + 1 < rank; ++i) gstride[i] = strides_bytes[i];
-  CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUtensorMapDataType dt = elem_bytes == 2   ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                           : elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                             : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = fn(map, dt, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim, gstride, bx, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

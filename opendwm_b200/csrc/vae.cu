@@ -1,7 +1,8 @@
 // HBM-bound kernels of the CogVideoX temporal-VAE decoder (channels-last activations):
 // GroupNorm statistics, the fused SpatialNorm3D (GroupNorm * conv_y(zq) + conv_b(zq)) +
-// SiLU that writes the 16-bit, causally time-padded input of the next convolution, and
-// the nearest-neighbour (space / space-time) upsampler.
+// SiLU that writes the 16-bit, causally time-padded input of the next convolution (or, for
+// the FP8 UNet ResBlock convs, its E4M3 version with one scale per volume), and the
+// nearest-neighbour (space / space-time) upsampler.
 #include <algorithm>
 
 #include "common.cuh"
@@ -132,7 +133,12 @@ struct SnParams {
   const float* zy; const float* zb; int Tz, hz, wz;
   int silu;
   void* out; int out_T, out_t0;
+  float* scale;   // E4M3 output: [nb] amax bits (SN_AMAX pass), then the volume scale
 };
+
+// What a spatialnorm_kernel pass does with each normalised float4: store it as 16 bit, only
+// fold it into the volume's amax, or store it as E4M3 with the volume's inverse scale.
+enum { SN_STORE16 = 0, SN_AMAX = 1, SN_E4M3 = 2 };
 
 // grid = (chunks, nb): a block works on one chunk (16 float4 per thread) of ONE image, so the (mean, rstd) of its
 // G groups are finalised once per block from the fp64 sums (first G threads, shared memory)
@@ -145,11 +151,12 @@ struct SnParams {
 // are powers of two apart (always in the VAEs) and the frame map is a 64-entry shared table.
 // A version that spent ~10 integer divisions per float4 was far from DRAM-bound; this one is
 // a plain stream.
-template <typename T>
+template <typename T, int MODE = SN_STORE16>
 __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, const int chunk) {
   // blockDim.x is a multiple of C/4 whenever C/4 <= 1024 (host side), `chunk` = blockDim.x * 16
   __shared__ float2 s_stat[64];
   __shared__ int s_tz[64];
+  __shared__ unsigned int s_amax;
   const int NT = static_cast<int>(blockDim.x);
   const int vec = p.C >> 2;
   const int n = blockIdx.y;
@@ -163,6 +170,7 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
     s_stat[threadIdx.x] = make_float2(static_cast<float>(mean_d),
                                       rsqrtf(static_cast<float>(ss / cnt - mean_d * mean_d) + p.eps));
   }
+  if (MODE == SN_AMAX && threadIdx.x == 0) s_amax = 0u;
   if (p.zy && threadIdx.x < 64 && threadIdx.x < p.T) {
     // nearest-neighbour frame of the latent grid; odd T > 1 treats the first frame apart
     const int t = threadIdx.x;
@@ -170,6 +178,30 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
                                      : (t * p.Tz) / p.T;
   }
   __syncthreads();
+  // SN_AMAX: max |v| of this thread, reduced per block in shared memory, then one atomicMax
+  // per block on the bits of the non-negative fp32 value (their integer order is the float
+  // order, so the result does not depend on the order of the atomics).  Blocks need not be
+  // whole warps (C/4 = 80 gives 240 threads), hence no warp shuffles.
+  float amax = 0.f;
+  float inv = 0.f;
+  if constexpr (MODE == SN_E4M3) inv = e4m3_inv(__uint_as_float(reinterpret_cast<const uint32_t*>(p.scale)[n]));
+  auto emit = [&](long long o, const float4& v) {
+    if constexpr (MODE == SN_STORE16) {
+      uint2 pk; pk.x = Cvt<T>::pack2(v.x, v.y); pk.y = Cvt<T>::pack2(v.z, v.w);
+      reinterpret_cast<uint2*>(p.out)[o] = pk;
+    } else if constexpr (MODE == SN_AMAX) {
+      amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+    } else {
+      reinterpret_cast<uint32_t*>(p.out)[o] = e4m3x4(v.x, v.y, v.z, v.w, inv);
+    }
+  };
+  auto finish = [&]() {
+    if constexpr (MODE == SN_AMAX) {
+      atomicMax(&s_amax, __float_as_uint(amax));
+      __syncthreads();
+      if (threadIdx.x == 0) atomicMax(reinterpret_cast<unsigned int*>(p.scale) + n, s_amax);
+    }
+  };
   const long long i0 = static_cast<long long>(blockIdx.x) * chunk;
   long long i1 = i0 + chunk;
   if (i1 > per_img) i1 = per_img;
@@ -219,11 +251,11 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
       }
       if (p.silu) { v.x = silu(v.x); v.y = silu(v.y); v.z = silu(v.z); v.w = silu(v.w); }
       const long long o = (((on + t) * p.H + h) * p.W + w) * vec + c4;
-      uint2 pk; pk.x = Cvt<T>::pack2(v.x, v.y); pk.y = Cvt<T>::pack2(v.z, v.w);
-      reinterpret_cast<uint2*>(p.out)[o] = pk;
+      emit(o, v);
       w += pstep;
       while (w >= p.W) { w -= p.W; if (++h == p.H) { h = 0; ++t; } }
     }
+    finish();
     return;
   }
   // general path (C / 4 > 1024 or more than 64 frames)
@@ -264,9 +296,15 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
     }
     if (p.silu) { v.x = silu(v.x); v.y = silu(v.y); v.z = silu(v.z); v.w = silu(v.w); }
     const long long o = (((static_cast<long long>(n) * p.out_T + p.out_t0 + t) * p.H + h) * p.W + w) * vec + c4;
-    uint2 pk; pk.x = Cvt<T>::pack2(v.x, v.y); pk.y = Cvt<T>::pack2(v.z, v.w);
-    reinterpret_cast<uint2*>(p.out)[o] = pk;
+    emit(o, v);
   }
+  finish();
+}
+
+// amax (bits, left in scale[] by the SN_AMAX pass) -> E4M3 volume scale
+__global__ void e4m3_amax_to_scale_kernel(float* scale, int nb) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n < nb) scale[n] = e4m3_scale(__uint_as_float(reinterpret_cast<const uint32_t*>(scale)[n]));
 }
 
 // ---- nearest upsample x2 in space, optionally in time (CogVideoXUpsample3D rules) ----
@@ -344,6 +382,7 @@ extern "C" int dwm_b200_spatialnorm_silu(const float* x, int64_t nb, int64_t T, 
   p.x = x; p.nb = (int)nb; p.T = (int)T; p.H = (int)H; p.W = (int)W; p.C = C; p.G = groups;
   p.sums = sums; p.eps = eps; p.gamma = gamma; p.beta = beta; p.zy = zy; p.zb = zb;
   p.Tz = Tz; p.hz = hz; p.wz = wz; p.silu = apply_silu; p.out = out; p.out_T = (int)out_T; p.out_t0 = (int)out_t0;
+  p.scale = nullptr;
   DWM_REQUIRE(groups <= 64 && nb <= 65535, "dwm_b200_spatialnorm_silu: groups <= 64 and nb <= 65535 required");
   const long long per_img = T * H * W * (C / 4);
   // block = the largest multiple of C/4 that fits 256 threads (or C/4 itself up to 1024), so a
@@ -357,6 +396,37 @@ extern "C" int dwm_b200_spatialnorm_silu(const float* x, int64_t nb, int64_t T, 
   if (dtype == DWM_BF16) spatialnorm_kernel<__nv_bfloat16><<<grid, threads, 0, s>>>(p, chunk);
   else if (dtype == DWM_F16) spatialnorm_kernel<__half><<<grid, threads, 0, s>>>(p, chunk);
   else { set_last_error("dwm_b200_spatialnorm_silu: bad dtype"); return -1; }
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dwm_b200_groupnorm_silu_e4m3(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C,
+                                            int groups, const double* sums, float eps, const float* gamma,
+                                            const float* beta, int apply_silu, void* out, int64_t out_T,
+                                            int64_t out_t0, float* out_scale, dwm_stream_t stream) {
+  DWM_REQUIRE(x && sums && gamma && beta && out && out_scale, "dwm_b200_groupnorm_silu_e4m3: null pointer");
+  DWM_REQUIRE(nb > 0 && T > 0 && H > 0 && W > 0, "dwm_b200_groupnorm_silu_e4m3: bad shape");
+  DWM_REQUIRE(C % 16 == 0 && groups > 0 && C % groups == 0 && groups <= 64,
+              "dwm_b200_groupnorm_silu_e4m3: need C %% 16 == 0, C %% groups == 0, groups <= 64 (got C=%d, groups=%d)",
+              C, groups);
+  DWM_REQUIRE(out_t0 >= 0 && out_t0 + T <= out_T, "dwm_b200_groupnorm_silu_e4m3: frame window outside out buffer");
+  DWM_REQUIRE(nb <= 65535, "dwm_b200_groupnorm_silu_e4m3: nb <= 65535 required");
+  SnParams p;
+  p.x = x; p.nb = (int)nb; p.T = (int)T; p.H = (int)H; p.W = (int)W; p.C = C; p.G = groups;
+  p.sums = sums; p.eps = eps; p.gamma = gamma; p.beta = beta; p.zy = nullptr; p.zb = nullptr;
+  p.Tz = p.hz = p.wz = 0; p.silu = apply_silu; p.out = out; p.out_T = (int)out_T; p.out_t0 = (int)out_t0;
+  p.scale = out_scale;
+  const long long per_img = T * H * W * (C / 4);
+  const int vec = C / 4;
+  int threads = 256;
+  if (vec <= 1024) threads = vec <= 256 ? (256 / vec) * vec : vec;
+  const int chunk = threads * 16;
+  dim3 grid(static_cast<unsigned>((per_img + chunk - 1) / chunk), static_cast<unsigned>(nb));
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  DWM_CHECK_CUDA(cudaMemsetAsync(out_scale, 0, sizeof(float) * nb, s));
+  spatialnorm_kernel<__nv_fp8_e4m3, SN_AMAX><<<grid, threads, 0, s>>>(p, chunk);
+  spatialnorm_kernel<__nv_fp8_e4m3, SN_E4M3><<<grid, threads, 0, s>>>(p, chunk);
+  e4m3_amax_to_scale_kernel<<<static_cast<unsigned>((nb + 127) / 128), 128, 0, s>>>(out_scale, (int)nb);
   DWM_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

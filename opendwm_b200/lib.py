@@ -88,6 +88,7 @@ class ConvArgs(ctypes.Structure):
         ("out", _p), ("ldo", _i64), ("resid", _p), ("ldr", _i64),
         ("resid_per_item", ctypes.c_int), ("rows_per_item", _i64),
         ("blend_x", _p), ("ldx", _i64), ("alpha", _p), ("rows_per_batch", _i64),
+        ("a_scale", _p), ("w_scale", _p),
     ]
 
 
@@ -127,6 +128,9 @@ SYMBOLS = {
         _p, _i64, _i64, _i64, _i64, ctypes.c_int, ctypes.c_int, _p, ctypes.c_float,
         _p, _p, _p, _p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _p,
         _i64, _i64, ctypes.c_int, _p]),
+    "dwm_b200_groupnorm_silu_e4m3": (ctypes.c_int, [
+        _p, _i64, _i64, _i64, _i64, ctypes.c_int, ctypes.c_int, _p, ctypes.c_float,
+        _p, _p, ctypes.c_int, _p, _i64, _i64, _p, _p]),
     "dwm_b200_upsample_nearest": (ctypes.c_int, [
         _p, _i64, _i64, _i64, _i64, ctypes.c_int, ctypes.c_int, _p, ctypes.c_int, _p]),
     "dwm_b200_euler_step_by_indices": (ctypes.c_int, [

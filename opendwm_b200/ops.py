@@ -413,11 +413,26 @@ def pack_conv_weight(weight: torch.Tensor, dtype, pad_out_to=None, pad_in_to=Non
     return w.to(dtype).contiguous()
 
 
+def pack_conv_weight_fp8(weight: torch.Tensor):
+    """torch Conv3d/Conv2d weight [O, I, (kt,) kh, kw] (on the GPU) -> (E4M3 tap-major
+    [kt*kh*kw, O, I], fp32 scale [O]).  Each output channel has ONE scale, the amax over all
+    of its taps and input channels: the [O, taps*I] view is quantized row-wise from fp32, then
+    stored tap-major like pack_conv_weight."""
+    if weight.dim() == 4:
+        weight = weight.unsqueeze(2)
+    o, i, kt, kh, kw = weight.shape
+    rows = weight.detach().float().permute(0, 2, 3, 4, 1).reshape(o, kt * kh * kw * i)
+    q, s = quantize_rows(rows.contiguous())
+    return q.view(o, kt * kh * kw, i).transpose(0, 1).contiguous(), s
+
+
 def conv(x, weight, bias=None, *, kernel, epilogue=_l.EPI_F32, act=_l.ACT_NONE,
          out=None, resid=None, resid_rows_per_item=0, blend_x=None, alpha=None,
-         rows_per_batch=0):
+         rows_per_batch=0, a_scale=None, w_scale=None):
     """x: 16-bit channels-last [nb, tp, h, w, c_in]; weight: tap-major
-    [kt*kh*kw, c_out, c_in]; returns [nb*(tp-kt+1)*h*w, c_out]."""
+    [kt*kh*kw, c_out, c_in]; returns [nb*(tp-kt+1)*h*w, c_out].
+    FP8: x and weight float8_e4m3fn with a_scale fp32 [nb] (one per volume,
+    groupnorm_silu_e4m3) and w_scale fp32 [c_out] (pack_conv_weight_fp8); RESID only."""
     if x.dim() != 5 or not x.is_contiguous() or not weight.is_contiguous():
         raise ValueError("conv: x must be contiguous [nb, tp, h, w, c]")
     if not x.is_cuda:
@@ -427,6 +442,18 @@ def conv(x, weight, bias=None, *, kernel, epilogue=_l.EPI_F32, act=_l.ACT_NONE,
     taps, c_out, c_in2 = weight.shape
     if taps != kt * kh * kw or c_in2 != c_in or weight.dtype != x.dtype:
         raise ValueError("conv: weight shape/dtype mismatch")
+    fp8 = x.dtype == FP8
+    if fp8:
+        if a_scale is None or w_scale is None:
+            raise ValueError("conv: FP8 operands need a_scale and w_scale")
+        if epilogue != _l.EPI_RESID:
+            raise ValueError("conv: FP8 operands need the RESID epilogue")
+        for t, n, name in ((a_scale, nb, "a_scale"), (w_scale, c_out, "w_scale")):
+            _f32(t, name)
+            if t.dim() != 1 or t.numel() != n:
+                raise ValueError("{} must be fp32 [{}]".format(name, n))
+    elif a_scale is not None or w_scale is not None:
+        raise ValueError("conv: a_scale / w_scale go with float8_e4m3fn operands")
     rows = nb * (tp - kt + 1) * h * w
     want = x.dtype if epilogue == _l.EPI_STORE else torch.float32
     if out is None:
@@ -438,7 +465,9 @@ def conv(x, weight, bias=None, *, kernel, epilogue=_l.EPI_F32, act=_l.ACT_NONE,
     a.x, a.nb, a.tp, a.h, a.w, a.c_in = x.data_ptr(), nb, tp, h, w, c_in
     a.weight, a.kt, a.kh, a.kw, a.c_out = weight.data_ptr(), kt, kh, kw, c_out
     a.bias = _ptr(_f32(bias, "bias"))
-    a.dtype, a.epilogue, a.act = _dt(x), epilogue, act
+    a.dtype, a.epilogue, a.act = _l.DWM_E4M3 if fp8 else _dt(x), epilogue, act
+    if fp8:
+        a.a_scale, a.w_scale = a_scale.data_ptr(), w_scale.data_ptr()
     a.out, a.ldo = out.data_ptr(), out.stride(0)
     if resid is not None:
         _rows2d(_f32(resid, "resid"), "resid")
@@ -485,6 +514,28 @@ def spatialnorm_silu(x, sums, gamma, beta, out, *, groups, eps=1e-6, zy=None,
         _ptr(zy), _ptr(zb), Tz, hz, wz, int(silu), out.data_ptr(), out.shape[1],
         out_t0, _dt(out), _stream()), "dwm_b200_spatialnorm_silu")
     return out
+
+
+def groupnorm_silu_e4m3(x, sums, gamma, beta, out, scale, *, groups, eps=1e-6, out_t0=0,
+                        silu=True):
+    """GroupNorm(+SiLU) of x fp32 [nb,T,H,W,C] into E4M3 out [nb,out_T,H,W,C] (frames
+    [out_t0, out_t0+T) only) with one fp32 scale per volume written to scale [nb]."""
+    _f32(x, "x")
+    if x.dim() != 5 or not x.is_contiguous():
+        raise ValueError("x must be contiguous [nb, T, H, W, C]")
+    nb, T, H, W, C = x.shape
+    if out.dtype != FP8 or out.dim() != 5 or not out.is_contiguous() or \
+            out.shape[0] != nb or out.shape[2:] != x.shape[2:]:
+        raise ValueError("out must be contiguous float8_e4m3fn [nb, out_T, H, W, C]")
+    _f32(scale, "scale")
+    if scale.numel() != nb or not scale.is_contiguous():
+        raise ValueError("scale must be fp32 [nb]")
+    _l.check(_l.load().dwm_b200_groupnorm_silu_e4m3(
+        x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), eps,
+        _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(), int(silu),
+        out.data_ptr(), out.shape[1], out_t0, scale.data_ptr(), _stream()),
+        "dwm_b200_groupnorm_silu_e4m3")
+    return out, scale
 
 
 def upsample_nearest(x, compress_time, dtype):

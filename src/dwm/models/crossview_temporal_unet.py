@@ -22,7 +22,8 @@ from opendwm_b200 import ops as _ops
 from .. import _compat
 from . import adapters as _adapters
 from .crossview_temporal import (
-    AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward)
+    AlphaBlender, ParamGroup, VTSelfAttentionBlock, fp8_operand, gemm, make_attention,
+    make_feed_forward)
 
 
 def _mlp(i, h, o):
@@ -187,8 +188,14 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                  enable_rowwise_temporal: bool = False,
                  condition_image_adapter_config=None, depth_net_config=None,
                  depth_frustum_range=None, enforce_align_projection=None,
-                 compute_dtype=None):
+                 compute_dtype=None, gemm_dtype=None):
+        """gemm_dtype=torch.float8_e4m3fn runs the ResBlock convolutions (spatial and temporal
+        conv1 / conv2) and the transformer-block linears (except the text K/V projections) in
+        E4M3; None keeps every GEMM and convolution 16-bit."""
         super().__init__()
+        if gemm_dtype not in (None, torch.float8_e4m3fn):
+            raise ValueError(
+                "gemm_dtype must be None or torch.float8_e4m3fn, got {!r}".format(gemm_dtype))
         if depth_net_config is not None or enforce_align_projection is not None:
             raise NotImplementedError(
                 "depth_net / align projection are not enabled by any shipped CTSD config")
@@ -209,6 +216,7 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                            block_out_channels=boc, cross_attention_dim=cross_attention_dim)
         self.in_channels, self.out_channels = in_channels, out_channels
         self.compute_dtype = compute_dtype
+        self.gemm_dtype = gemm_dtype
         self.norm_eps = norm_eps
         self.gradient_checkpointing = False
         self.conv_in = torch.nn.Conv2d(in_channels, boc[0], 3, padding=1)
@@ -248,6 +256,7 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         self._pk = None
         self._cond_key = None
         self._cond = None
+        self._ws8, self._ws8_key = {}, None
 
     # -- plumbing ---------------------------------------------------------------------------
     def enable_gradient_checkpointing(self):
@@ -255,10 +264,12 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
 
     def _apply(self, fn, *a, **k):
         self._pk, self._cond_key, self._cond = None, None, None
+        self._ws8, self._ws8_key = {}, None
         return super()._apply(fn, *a, **k)
 
     def load_state_dict(self, state_dict, strict=True, assign=False):
         self._pk, self._cond_key, self._cond = None, None, None
+        self._ws8, self._ws8_key = {}, None
         return super().load_state_dict(state_dict, strict=strict, assign=assign)
 
     def _dtype(self):
@@ -275,6 +286,7 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             raise RuntimeError("UNetCrossviewTemporalConditionModel runs on CUDA (sm_90a) "
                                "only; there is no CPU fallback. Move the model to the GPU.")
         dt = self._dtype()
+        fp8 = self.gemm_dtype is not None
 
         def f32(t):
             return t.detach().to(dev, torch.float32).contiguous()
@@ -282,6 +294,21 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         def lin(m):
             return (m.weight.detach().to(dev, dt).contiguous(),
                     None if m.bias is None else f32(m.bias))
+
+        def lin8(w, b):
+            """`gemm` weight tuple of a block linear: E4M3 + channel scales with gemm_dtype,
+            else 16-bit (b: fp32 or None)."""
+            if not fp8:
+                return w.detach().to(dev, dt).contiguous(), b
+            w8, s = _ops.quantize_weight_rows(w.to(dev))
+            return w8, b, s, dt
+
+        def conv8(m):
+            """A ResBlock conv: E4M3 tap-major weight + bias + channel scales with gemm_dtype."""
+            if not fp8:
+                return conv(m)
+            w8, s = _ops.pack_conv_weight_fp8(m.weight.to(dev))
+            return w8, f32(m.bias), s
 
         def conv(m, pad_out=None, pad_in=None):
             w = _ops.pack_conv_weight(m.weight.to(dev), dt, pad_out_to=pad_out, pad_in_to=pad_in)
@@ -306,16 +333,16 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
 
         def res(rb):
             s = rb.spatial_res_block
-            p = dict(n1=gn(s.norm1), c1=conv(s.conv1), temb=temb_slot(s.time_emb_proj),
-                     n2=gn(s.norm2), c2=conv(s.conv2))
+            p = dict(n1=gn(s.norm1), c1=conv8(s.conv1), temb=temb_slot(s.time_emb_proj),
+                     n2=gn(s.norm2), c2=conv8(s.conv2))
             if hasattr(s, "conv_shortcut"):
                 c = s.conv_shortcut
                 p["sc"] = (c.weight.detach().reshape(c.out_channels, -1).to(dev, dt).contiguous(),
                            f32(c.bias))
             if rb.temporal_res_block is not None:
                 t = rb.temporal_res_block
-                p["t"] = dict(n1=gn(t.norm1), c1=conv(t.conv1), temb=temb_slot(t.time_emb_proj),
-                              n2=gn(t.norm2), c2=conv(t.conv2))
+                p["t"] = dict(n1=gn(t.norm1), c1=conv8(t.conv1), temb=temb_slot(t.time_emb_proj),
+                              n2=gn(t.norm2), c2=conv8(t.conv2))
             return p
 
         def attn(tm):
@@ -323,27 +350,30 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                      blocks=[])
             for b in tm.transformer_blocks:
                 a1, a2 = b.attn1, b.attn2
+
+                def blin(m):
+                    return lin8(m.weight.detach(), None if m.bias is None else f32(m.bias))
+                ff1_w, ff1_b = _ops.pack_geglu(b.ff.net[0].proj.weight.detach().to(dev),
+                                               b.ff.net[0].proj.bias.detach().to(dev))
                 p["blocks"].append(dict(
                     n1=(f32(b.norm1.weight), f32(b.norm1.bias), b.norm1.eps),
-                    qkv=torch.cat([a1.to_q.weight, a1.to_k.weight, a1.to_v.weight])
-                    .detach().to(dev, dt).contiguous(),
-                    out=lin(a1.to_out[0]),
+                    qkv=lin8(torch.cat([a1.to_q.weight, a1.to_k.weight, a1.to_v.weight])
+                             .detach(), None),
+                    out=blin(a1.to_out[0]),
                     n2=(f32(b.norm2.weight), f32(b.norm2.bias), b.norm2.eps),
-                    q2=lin(a2.to_q),
+                    q2=blin(a2.to_q),
                     kv2=torch.cat([a2.to_k.weight, a2.to_v.weight]).detach().to(dev, dt).contiguous(),
-                    out2=lin(a2.to_out[0]),
+                    out2=blin(a2.to_out[0]),
                     n3=(f32(b.norm3.weight), f32(b.norm3.bias), b.norm3.eps),
-                    ff1=_ops.pack_geglu(b.ff.net[0].proj.weight.detach().to(dev),
-                                        b.ff.net[0].proj.bias.detach().to(dev)),
-                    ff2=lin(b.ff.net[2])))
-                q = p["blocks"][-1]
-                q["ff1"] = (q["ff1"][0].to(dt).contiguous(), q["ff1"][1].float().contiguous())
+                    # FP8: quantized after the GEGLU row packing, scales follow the rows
+                    ff1=lin8(ff1_w, ff1_b.float().contiguous()),
+                    ff2=blin(b.ff.net[2])))
             if tm.view_pos_embed is not None:
                 p["vpe"] = (lin(tm.view_pos_embed.linear_1), lin(tm.view_pos_embed.linear_2))
-                p["cv"] = [b.pack(dt, dev) for b in tm.crossview_transformer_blocks]
+                p["cv"] = [b.pack(dt, dev, fp8) for b in tm.crossview_transformer_blocks]
             if tm.time_pos_embed is not None:
                 p["tpe"] = (lin(tm.time_pos_embed.linear_1), lin(tm.time_pos_embed.linear_2))
-                p["tp"] = [b.pack(dt, dev) for b in tm.temporal_transformer_blocks]
+                p["tp"] = [b.pack(dt, dev, fp8) for b in tm.temporal_transformer_blocks]
             return p
 
         def block(b):
@@ -356,7 +386,7 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             return p
 
         cin_p = (self.in_channels + 7) // 8 * 8
-        pk = dict(dtype=dt, cin_p=cin_p,
+        pk = dict(dtype=dt, fp8=fp8, cin_p=cin_p,
                   conv_in=conv(self.conv_in, pad_in=cin_p),
                   te=(lin(self.time_embedding.linear_1), lin(self.time_embedding.linear_2)),
                   down=[block(b) for b in self.down_blocks], mid=block(self.mid_block),
@@ -380,20 +410,53 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         _ops.spatialnorm_silu(h5, sums, g[0], g[1], out, groups=32, eps=g[2], silu=silu)
         return out
 
+    def _buf8(self, key, shape, dtype):
+        """E4M3 workspace (operands, volume scales) kept across calls of one input geometry,
+        so that a CUDA-graph replay reads and writes the buffers the capture recorded.  The
+        buffers start zeroed: the temporal convs rely on zero cache frames."""
+        k = (key, tuple(shape), dtype)
+        if k not in self._ws8:
+            self._ws8[k] = torch.zeros(shape, device=self.conv_in.weight.device, dtype=dtype)
+        return self._ws8[k]
+
+    def _gn8(self, x5, g, out_T=None, out_t0=0):
+        """GroupNorm(32)+SiLU of fp32 [nb, T, H, W, C] as an FP8 conv operand: (E4M3
+        [nb, out_T, H, W, C], fp32 scales [nb]), one scale per volume nb.  Frames outside
+        [out_t0, out_t0 + T) stay zero."""
+        nb, T, H, W, C = x5.shape
+        out_T = T if out_T is None else out_T
+        sums = _ops.groupnorm_stats(x5, 32)
+        out = self._buf8("gn", (nb, out_T, H, W, C), torch.float8_e4m3fn)
+        sc = self._buf8("gn_s", (nb,), torch.float32)
+        return _ops.groupnorm_silu_e4m3(x5, sums, g[0], g[1], out, sc, groups=32, eps=g[2],
+                                        out_t0=out_t0, silu=True)
+
+    @staticmethod
+    def _conv(a, c, **kw):
+        """ResBlock conv of operand `a` (16-bit, or _gn8's (E4M3, scales)) with packed c."""
+        if len(c) == 3:
+            return _ops.conv(a[0], c[0], c[1], a_scale=a[1], w_scale=c[2], **kw)
+        return _ops.conv(a, *c, **kw)
+
     def _resblock(self, p, h, N, H, W, temb_all, geo, dis_t, alpha_mod):
         S = H * W
-        a = self._gn(h, N, H, W, p["n1"], True)
+
+        def norm_act(t, g):    # conv operand: 16-bit, or E4M3 with one scale per item
+            if self._pk["fp8"]:
+                return self._gn8(t.view(N, 1, H, W, t.shape[1]), g)
+            return self._gn(t, N, H, W, g, True)
+        a = norm_act(h, p["n1"])
         o, n = p["temb"]
-        h1 = _ops.conv(a, *p["c1"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID,
-                       resid=temb_all[:, o:o + n], resid_rows_per_item=S)
-        b = self._gn(h1, N, H, W, p["n2"], True)
+        h1 = self._conv(a, p["c1"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID,
+                        resid=temb_all[:, o:o + n], resid_rows_per_item=S)
+        b = norm_act(h1, p["n2"])
         if "sc" in p:
             h16 = torch.empty(h.shape, device=h.device, dtype=self._pk["dtype"])
             _ops.act_cast(h, h16)
             skip = _ops.linear(h16, *p["sc"], epilogue=_lib.EPI_F32)
         else:
             skip = h
-        out = _ops.conv(b, *p["c2"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID, resid=skip)
+        out = self._conv(b, p["c2"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID, resid=skip)
         if "t" in p and not dis_t["all"]:
             out = self._temporal_res(p["t"], out, N, H, W, temb_all, geo, alpha_mod)
         return out
@@ -410,18 +473,20 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             .reshape(B * V * T, n).contiguous()
 
         def norm_act(t5, g):
+            if self._pk["fp8"]:     # E4M3 with one scale per (b v) volume of T frames
+                return self._gn8(t5, g, out_T=T + 2, out_t0=1)
             sums = _ops.groupnorm_stats(t5, 32)
             buf = torch.zeros(B * V, T + 2, 1, S, C, device=x.device, dtype=dt)
             _ops.spatialnorm_silu(t5, sums, g[0], g[1], buf, groups=32, eps=g[2], out_t0=1,
                                   silu=True)
             return buf
-        h1 = _ops.conv(norm_act(x5, p["n1"]), *p["c1"], kernel=(3, 1, 1),
-                       epilogue=_lib.EPI_RESID, resid=temb_p, resid_rows_per_item=S)
+        h1 = self._conv(norm_act(x5, p["n1"]), p["c1"], kernel=(3, 1, 1),
+                        epilogue=_lib.EPI_RESID, resid=temb_p, resid_rows_per_item=S)
         xr = xp.view(B * V * T * S, C)
         alpha = mixer["alpha"]
-        y = _ops.conv(norm_act(h1.view(B * V, T, 1, S, C), p["n2"]), *p["c2"],
-                      kernel=(3, 1, 1), epilogue=_lib.EPI_RESID, resid=xr, blend_x=xr,
-                      alpha=alpha, rows_per_batch=V * T * S)
+        y = self._conv(norm_act(h1.view(B * V, T, 1, S, C), p["n2"]), p["c2"],
+                       kernel=(3, 1, 1), epilogue=_lib.EPI_RESID, resid=xr, blend_x=xr,
+                       alpha=alpha, rows_per_batch=V * T * S)
         return y.view(B, V, T, S, C).permute(0, 2, 1, 3, 4).reshape(B * T * V * S, C)\
             .contiguous()
 
@@ -443,6 +508,26 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                   g16=torch.empty(N * S, 4 * inner, device=dev, dtype=dt),
                   qkv_s=torch.empty(N * S, 3 * inner, device=dev, dtype=dt),
                   o16=torch.empty(N * S, inner, device=dev, dtype=dt))
+        fp8 = self._pk["fp8"]
+        if fp8:
+            # E4M3 operands + row scales: LayerNorm outputs (a8) and the quantized 16-bit
+            # attention / GEGLU outputs (q8); the VTSelfAttentionBlocks use the same keys
+            f8 = torch.float8_e4m3fn
+            for k, cols in (("a8", inner), ("q8", 4 * inner)):
+                ws[k] = self._buf8(k, (N * S, cols), f8)
+                ws[k + "_s"] = self._buf8(k + "_s", (N * S,), torch.float32)
+            a = (ws["a8"], ws["a8_s"])
+        else:
+            a = ws["a16"]
+
+        def ln(src, g):
+            if fp8:
+                _ops.layernorm(src, a[0], out_scale=a[1], weight=g[0], bias=g[1], eps=g[2])
+            else:
+                _ops.layernorm(src, a, weight=g[0], bias=g[1], eps=g[2])
+
+        def operand(t):    # the 16-bit GEMM output t as the next GEMM's operand
+            return fp8_operand(ws, "q8", t) if fp8 else t
         ctx = cd["ctx16"]
         Lc = cd["ctx_len"]
         key = (level_key, "tabs")
@@ -460,13 +545,13 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         tabs = cd[key]
         for li, bp in enumerate(p["blocks"]):
             # --- spatial BasicTransformerBlock: self-attn, cross-attn to text, GEGLU FF
-            _ops.layernorm(h, ws["a16"], weight=bp["n1"][0], bias=bp["n1"][1], eps=bp["n1"][2])
-            _ops.linear(ws["a16"], bp["qkv"], None, out=ws["qkv_s"])
+            ln(h, bp["n1"])
+            gemm(a, bp["qkv"], out=ws["qkv_s"])
             _ops.attention(ws["qkv_s"], ws["o16"], D=inner, heads=heads, group_dims=[N],
                            group_strides=[S], seq=S)
-            _ops.linear(ws["o16"], *bp["out"], epilogue=_lib.EPI_RESID, resid=h, out=h)
-            _ops.layernorm(h, ws["a16"], weight=bp["n2"][0], bias=bp["n2"][1], eps=bp["n2"][2])
-            q = _ops.linear(ws["a16"], *bp["q2"], out=ws["qkv_s"][:, :inner])
+            gemm(operand(ws["o16"]), bp["out"], epilogue=_lib.EPI_RESID, resid=h, out=h)
+            ln(h, bp["n2"])
+            q = gemm(a, bp["q2"], out=ws["qkv_s"][:, :inner])
             kkey = (level_key, li, "kv")
             if kkey not in cd:        # text K,V are step-invariant
                 cd[kkey] = _ops.linear(ctx, bp["kv2"], None)
@@ -474,10 +559,10 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             _ops.attention(q, ws["o16"], D=inner, heads=heads, group_dims=[N],
                            group_strides=[S], seq=S, kv=kv, k_col=0, v_col=inner,
                            kv_group_strides=[Lc], seq_kv=Lc)
-            _ops.linear(ws["o16"], *bp["out2"], epilogue=_lib.EPI_RESID, resid=h, out=h)
-            _ops.layernorm(h, ws["a16"], weight=bp["n3"][0], bias=bp["n3"][1], eps=bp["n3"][2])
-            _ops.linear(ws["a16"], *bp["ff1"], epilogue=_lib.EPI_GEGLU, out=ws["g16"])
-            _ops.linear(ws["g16"], *bp["ff2"], epilogue=_lib.EPI_RESID, resid=h, out=h)
+            gemm(operand(ws["o16"]), bp["out2"], epilogue=_lib.EPI_RESID, resid=h, out=h)
+            ln(h, bp["n3"])
+            gemm(a, bp["ff1"], epilogue=_lib.EPI_GEGLU, out=ws["g16"])
+            gemm(operand(ws["g16"]), bp["ff2"], epilogue=_lib.EPI_RESID, resid=h, out=h)
             # --- cross-view block
             if "cv" in p and not cd["dis_cv"]["all"]:
                 if tm.enable_rowwise_crossview:   # (bt h) x (v w), view mask per (vq, vk)
@@ -629,6 +714,8 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         pk, dt = self._pk, self._pk["dtype"]
         B, T, V, Cin, H, W = sample.shape
         N, geo, dev = B * T * V, (B, T, V), sample.device
+        if self._ws8_key != (B, T, V, H, W):     # one live E4M3 workspace
+            self._ws8, self._ws8_key = {}, (B, T, V, H, W)
         cd = self._conditions(geo, H, W, encoder_hidden_states, condition_image_tensor,
                               added_time_ids, disable_crossview, disable_temporal,
                               crossview_attention_mask)
