@@ -11,8 +11,8 @@
 //                  the tile and then applies the fused epilogue straight from its register
 //                  fragment (E4M3: after scaling it by the row and channel scales)
 // A stage is 128 bytes of K per row in either case: 64 16-bit or 128 E4M3 elements.
-// NT = 256 (the widest wgmma; 128 accumulator registers per thread) unless a 128-wide tile
-// gives the last wave fewer idle SMs.
+// NT = 256 (the widest wgmma; 128 accumulator registers per thread) unless the 256-wide tiles
+// leave most SMs idle (pick_tile_n).
 //
 // Replaces the cuBLASLt GEMM + ~10 elementwise launches per sub-layer that the
 // reference runs (SURVEY.md §2.3 K5-K8).
@@ -174,16 +174,19 @@ static int launch_gemm(const dwm_linear_args* a, cudaStream_t stream) {
 int g_gemm_bn = 0;   // 0: tile width by wave efficiency; 128 / 256 force it (option "gemm_bn")
 int g_gemm_2cta = -1;   // -1: from env DWM_GEMM_2CTA (default 1), 0 / 1: forced (option "gemm_2cta")
 
-// Time of a persistent launch ~ waves x tile width: the 128-wide tile wins when the 256-wide
-// tiles leave a last wave that is mostly idle SMs.
+// Time of a persistent launch ~ waves x tile width / rate.  A 128-wide tile streams 1.5x the
+// A + W bytes from L2 per FLOP of a 256-wide one, and with every SM busy it runs at about 0.6 of
+// its rate (H100 80GB HBM3 at 700 W, 86016-row fp16 STORE GEMMs, K = 1536: 250 against 420
+// TFLOP/s).  So the 128-wide tile wins only when the 256-wide tiles leave most SMs idle, not
+// for the fraction of a wave that the tile count rounds off.
 static int pick_tile_n(const dwm_linear_args* a, int cl) {
   if (a->epilogue == DWM_EPI_GEGLU) return 256;
   if (g_gemm_bn == 128 || g_gemm_bn == 256) return g_gemm_bn;
   const long long slots = sm_count() / cl;
   const long long m_groups = ((a->M + BM - 1) / BM + cl - 1) / cl;
   const long long t256 = m_groups * ((a->N + 255) / 256), t128 = m_groups * ((a->N + 127) / 128);
-  const long long cost256 = ((t256 + slots - 1) / slots) * 256, cost128 = ((t128 + slots - 1) / slots) * 128;
-  return cost128 < cost256 ? 128 : 256;
+  const long long waves256 = (t256 + slots - 1) / slots, waves128 = (t128 + slots - 1) / slots;
+  return waves128 * 128 * 5 < waves256 * 256 * 3 ? 128 : 256;   // 128-wide cost / 0.6
 }
 
 template <typename TA, typename T, int EPI, int CL>
