@@ -144,7 +144,10 @@ int dwm_b200_linear(const dwm_linear_args* args, dwm_stream_t stream);
  * q = cols [h*64, h*64+64), k = D + ..., v = 2D + ....  Output rows use the out_* strides;
  * with split > 0, positions j >= split go to out2 row g*(seq-split) + (j-split)
  * (context tokens of the joint attention).  mask: uint8 [batches, n_outer, n_outer],
- * entry [g0 / mask_div, jq / inner, jk / inner] != 0 means "attend".
+ * entry [g0 / mask_div, jq / inner, jk / inner] != 0 means "attend".  A query whose every
+ * key is masked gets an output of 0 (F.scaled_dot_product_attention gives NaN there; a NaN
+ * would spread through the whole residual stream).  Rows of qkv that no sequence position
+ * maps to (padding between groups) are never used and may hold anything, NaN included.
  * Replaces F.scaled_dot_product_attention inside diffusers AttnProcessor2_0 /
  * JointAttnProcessor2_0 and the einops regroupings of
  * crossview_temporal_dit.py:300-315 (cross-view rowwise + mask expansion) and :335-361

@@ -297,7 +297,8 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
         const int row = rows[hi];
         const int j = qt * BQ + row;
         if (!(G ? row_ok[hi] : (j < p.seq))) continue;
-        const float inv = 1.0f / l[hi];
+        // a query whose every key is masked (G only) has l = 0 and O = 0: write 0, not 0 * inf
+        const float inv = l[hi] > 0.f ? 1.0f / l[hi] : 0.f;
         T* dst;
         if constexpr (G) {
           const int g0 = g / p.g1n, i1 = g - g0 * p.g1n;
@@ -383,10 +384,14 @@ static int launch_attn_wgmma(const dwm_attention_args* a, cudaStream_t s) {
 }
 
 // contiguous, unmasked head_dim-64 sequences (joint / dual attention, UNet spatial attention)
+// packed back to back: the 2-D tensor map loads whole 128-row K / V blocks, so the rows after a
+// sequence must be the next sequence or the map's zero fill.  Padding rows between sequences
+// could hold anything, and P = 0 times a NaN / Inf there would still reach O; such layouts go to
+// the mma.sync kernel, which zero-fills out-of-sequence rows.
 bool attn_tc_eligible(const dwm_attention_args* a) {
   return a->kv == nullptr && a->mask == nullptr && a->group_dims[1] == 1 && a->group_dims[2] == 1 &&
          a->inner == a->seq && a->stride_inner == 1 && a->out_stride_inner == 1 && a->seq > 64 &&
-         a->group_strides[0] >= a->seq && a->group_dims[0] * a->group_strides[0] < (1ll << 31);
+         a->group_strides[0] == a->seq && a->group_dims[0] * a->group_strides[0] < (1ll << 31);
 }
 
 // gathered sequences of whole units of `inner` contiguous tokens (cross-view / temporal
