@@ -448,7 +448,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         if self.__dict__.pop("_ring_shift", False) and self._ring_applicable(
                 B, T, V, Hp, Wp, t_offset, T_total, condition_image_tensor):
             cd = self._conditions_shifted(
-                B, T, V, Hp, Wp, encoder_hidden_states, pooled_projections,
+                B, T, V, Hp, Wp, t_offset, T_total, encoder_hidden_states, pooled_projections,
                 condition_image_tensor, added_time_ids, disable_crossview, disable_temporal,
                 crossview_attention_mask)
             self._cond_key, self._cond, self._cond_refs = key, cd, refs
@@ -526,22 +526,28 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
 
     # -- streaming ring update of the step-invariant cache (opt-in, SURVEY.md §8(f)2) -----------
     def _ring_applicable(self, B, T, V, Hp, Wp, t_offset, T_total, image):
+        """T frames from t_offset of a T_total-frame window: the whole window on one GPU, or
+        a frame shard (`ShardPlan`) of it."""
         old = self._cond
-        return old is not None and T > 1 and t_offset == 0 and T_total == T and \
-            old.get("_geom") == (B, T, V, Hp, Wp, 0, T) and \
+        return old is not None and T > 1 and \
+            old.get("_geom") == (B, T, V, Hp, Wp, t_offset, T_total) and \
             (image is None or image.shape[1] == T)
 
-    def _conditions_shifted(self, B, T, V, Hp, Wp, ehs, pooled, image, ids, dis_cv, dis_t, mask):
+    def _conditions_shifted(self, B, T, V, Hp, Wp, t_offset, T_total, ehs, pooled, image, ids,
+                            dis_cv, dis_t, mask):
         """The FIFO moved on by one frame: every per-item entry of the cached condition set is
         the old one shifted by a frame, only the last frame's entries (context embedding, pooled
         text MLP, camera embedding, ImageAdapter residuals) are computed.  The index-embedding
-        sums are re-formed because a frame's time index changes with its queue slot."""
+        sums are re-formed because a frame's time index changes with its queue slot.
+
+        A frame shard shifts the same way: its new last slot is window frame
+        t_offset + T - 1, computed from the shard's own conditions, so no exchange is needed."""
         old = self._cond
         saved = (self._cond_key, self._cond)
         self._cond_key = None
         one = lambda t: None if t is None else t[:, T - 1:]          # noqa: E731
-        cd1 = self._conditions(B, 1, V, Hp, Wp, T - 1, T, one(ehs), one(pooled), one(image),
-                               one(ids), dis_cv, dis_t, mask)
+        cd1 = self._conditions(B, 1, V, Hp, Wp, t_offset + T - 1, T_total, one(ehs), one(pooled),
+                               one(image), one(ids), dis_cv, dis_t, mask)
         self._cond_key, self._cond = saved
 
         def shift(o, n):
@@ -556,7 +562,8 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         cd["text_emb"] = shift(old["text_emb"], cd1["text_emb"])
         view_cam = cd["_view_cam"] = shift(old["_view_cam"], cd1["_view_cam"])
         dev = cd["c0"].device
-        item_t = torch.arange(T, device=dev).view(1, T, 1).expand(B, T, V).reshape(-1)
+        item_t = (torch.arange(T, device=dev) + t_offset).view(1, T, 1)\
+            .expand(B, T, V).reshape(-1)
         item_v = torch.arange(V, device=dev).view(1, 1, V).expand(B, T, V).reshape(-1)
         if self.enable_temporal:
             cd["temb_tab"] = []

@@ -355,12 +355,19 @@ class CrossviewTemporalSD:
             self.generator.manual_seed(box[0])
 
     # -- the fused denoising step ----------------------------------------------------------
-    def _df_step_tensors(self, i, T, spi, take_time, B, V):
+    def _df_step_tensors(self, i, T, spi, take_time, B, V, frames=None):
         """Device-resident index tensors of one diffusion-forcing step, cached per
         (i, take_time): the reference rebuilds them from Python lists every step
-        (:2048-2055, :2083-2088)."""
-        key = (i, T, spi, take_time, B, V, self.test_scheduler.num_inference_steps)
+        (:2048-2055, :2083-2088).  `frames` (a `ShardPlan.frame_slice()`) caches this
+        rank's frames of them instead."""
+        key = (i, T, spi, take_time, B, V, self.test_scheduler.num_inference_steps,
+               None if frames is None else (frames.start, frames.stop))
         hit = self._step_cache.get(key)
+        if hit is None and frames is not None:
+            idx, timesteps, in_range = self._df_step_tensors(i, T, spi, take_time, B, V)
+            hit = (idx[:, frames].contiguous(), timesteps[:, frames].contiguous(),
+                   in_range[frames].contiguous())
+            self._step_cache[key] = hit
         if hit is None:
             idx = torch.tensor(
                 _ti.df_timestep_indices(i, T, spi, take_time),
@@ -835,25 +842,62 @@ class StreamingCrossviewTemporalSD(CrossviewTemporalSD):
             self.inference_config["inference_steps"], self.device)
         self.prev_ego_transforms = None
         self._step_cache = {}
+        self._local_conditions = None
+        self._streaming_plan()
+
+    def _streaming_plan(self):
+        """The ShardPlan of the streaming steps, or None.  Sharding is DiT-only: a UNet
+        pipeline with a plan is refused rather than run unsharded on every rank."""
+        plan = self.sharding
+        if plan is not None and not self.is_dit:
+            raise NotImplementedError(
+                "StreamingCrossviewTemporalSD.sharding needs the DiT model: the CTSD-2.1 UNet "
+                "step is not sharded; detach the ShardPlan (pipe.sharding = None)")
+        return plan
 
     @torch.no_grad()
     def inference_pipeline(self, latent_shape, start_timestep: int = 0,
                            stop_timestep=None, take_time: int = 0):
-        """reference :2031-2103."""
+        """reference :2031-2103.
+
+        With a ShardPlan every rank holds the whole FIFO (`self.latents`, `self.conditions`);
+        a call runs its steps on this rank's CFG branch and frames and all-gathers the FIFO
+        once at the end.  The exiting frame's views are decoded item-parallel over all
+        ranks, so every rank emits the same frame."""
         steps = self.inference_config["inference_steps"]
         assert steps % latent_shape[1] == 0
         spi = steps // latent_shape[1]
         B, T, V = latent_shape[:3]
         latents = self.latents.to(torch.float32).contiguous()
         stop_timestep = stop_timestep or steps
+        plan = self._streaming_plan()
+        conditions, fs, decode, work = self.conditions, None, self.decode_latents, latents
+        if plan is not None:
+            if plan.T != T:
+                raise ValueError("the ShardPlan splits {} frames, the FIFO holds {}".format(
+                    plan.T, T))
+            # sliced once per condition update: the flush reuses one condition set, and the
+            # model's condition cache is keyed by tensor address
+            if self._local_conditions is None or self._local_conditions[0] is not plan:
+                self._local_conditions = (plan, plan.local_conditions(
+                    self.conditions, cfg_doubled="guidance_scale" in self.inference_config))
+            conditions, fs = self._local_conditions[1], plan.frame_slice()
+            work = plan.local_latents(latents)
+            if self.vae is not None:
+                decode = lambda t: plan.split_call(self.decode_latents, t)  # noqa: E731
         for i in range(start_timestep, stop_timestep):
             idx, timesteps, in_range = self._df_step_tensors(
-                i, T, spi, take_time, B, V)
-            self.denoise_step(latents, self.conditions, idx, timesteps, in_range)
+                i, T, spi, take_time, B, V, frames=fs)
+            self.denoise_step(work, conditions, idx, timesteps, in_range)
+        if plan is not None:
+            # unsharded, the steps update `latents` in place, and an fp32 FIFO is `latents`
+            # itself (so in the flush its finished slots keep the extra steps): the gathered
+            # FIFO goes to the same tensor, and both paths leave the same `self.latents`
+            latents.copy_(plan.gather_latents(work))
         if stop_timestep >= steps:
             # reference :2092-2101: VAE decode of the exiting frame, then
             # image_processor.postprocess(image_tensor, self.output_type)
-            image_tensor = self.decode_latents(latents[:, take_time].flatten(0, 1))
+            image_tensor = decode(latents[:, take_time].flatten(0, 1))
             self.frames.append(
                 image_tensor if self.vae is None else
                 CrossviewTemporalSD.postprocess(image_tensor, self.output_type))
@@ -898,6 +942,7 @@ class StreamingCrossviewTemporalSD(CrossviewTemporalSD):
         keep = self.inference_config[
             "autoregression_condition_exception_for_take_sequence"]
         noise_scale = getattr(self.test_scheduler, "init_noise_sigma", 1)
+        self._local_conditions = None          # a ShardPlan re-slices the new condition set
         if self.condition_count < seq:        # gathering
             for k, v in fc.items():
                 if k not in self.conditions or k in keep or v is None:
