@@ -175,8 +175,15 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) 
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
   return r;
 }
+// Arrive on an mbarrier of another CTA of the cluster, without cluster-scope release semantics.
+// The only use is a consumer telling the peer's producer that this CTA has finished READING a
+// stage, so the peer's next multicast may overwrite it.  Those reads were made by wgmma and are
+// complete once wgmma.wait_group returns; no write of this thread has to become visible to the
+// peer.  ".release.cluster" would make ptxas put MEMBAR.ALL.GPU in front of the arrive, which
+// waits for every earlier store of the warp (the previous tile's epilogue) inside the k-loop.
+// The plain form (default .release.cta) is a bare SYNCS.ARRIVE.TRANS64.RED.
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 // 2-D tile load written to the same shared-memory offset of every CTA in `mask`; each
 // destination's mbarrier at the offset of `bar` receives the transaction bytes

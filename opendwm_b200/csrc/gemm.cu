@@ -175,10 +175,11 @@ int g_gemm_bn = 0;   // 0: tile width by wave efficiency; 128 / 256 force it (op
 int g_gemm_2cta = -1;   // -1: from env DWM_GEMM_2CTA (default 1), 0 / 1: forced (option "gemm_2cta")
 
 // Time of a persistent launch ~ waves x tile width / rate.  A 128-wide tile streams 1.5x the
-// A + W bytes from L2 per FLOP of a 256-wide one, and with every SM busy it runs at about 0.6 of
-// its rate (H100 80GB HBM3 at 700 W, 86016-row fp16 STORE GEMMs, K = 1536: 250 against 420
-// TFLOP/s).  So the 128-wide tile wins only when the 256-wide tiles leave most SMs idle, not
-// for the fraction of a wave that the tile count rounds off.
+// A + W bytes from L2 per FLOP of a 256-wide one, and with every SM busy it runs at about 0.9 of
+// its rate (tools/gemm_bench.py on an H100 80GB HBM3 at 400 W, the step's 86016- and 29568-row
+// shapes, fp16 and bf16: median 0.92-0.94, range 0.82-1.12).  So the 128-wide tile wins when
+// it saves a tenth of the waves x width, not for a smaller fraction of a wave that the tile
+// count rounds off: 4096 x 1536 x 1536 RESID picks 128 (1.1-1.3x), 2048 x 1536 keeps 256.
 static int pick_tile_n(const dwm_linear_args* a, int cl) {
   if (a->epilogue == DWM_EPI_GEGLU) return 256;
   if (g_gemm_bn == 128 || g_gemm_bn == 256) return g_gemm_bn;
@@ -186,7 +187,7 @@ static int pick_tile_n(const dwm_linear_args* a, int cl) {
   const long long m_groups = ((a->M + BM - 1) / BM + cl - 1) / cl;
   const long long t256 = m_groups * ((a->N + 255) / 256), t128 = m_groups * ((a->N + 127) / 128);
   const long long waves256 = (t256 + slots - 1) / slots, waves128 = (t128 + slots - 1) / slots;
-  return waves128 * 128 * 5 < waves256 * 256 * 3 ? 128 : 256;   // 128-wide cost / 0.6
+  return waves128 * 128 * 10 < waves256 * 256 * 9 ? 128 : 256;   // 128-wide cost / 0.9
 }
 
 template <typename TA, typename T, int EPI, int CL>
@@ -278,7 +279,11 @@ extern "C" int dwm_b200_linear(const dwm_linear_args* a, dwm_stream_t stream) {
     const char* e = getenv("DWM_GEMM_2CTA");
     g_gemm_2cta = (e && e[0] == '0') ? 0 : 1;
   }
-  // pairs pay off once there are enough 128-row tiles to give both CTAs of a cluster work
+  // Pairs halve the W traffic from L2, which pays at large K (8192^3: 1.25-1.4x, K = 6144: up
+  // to 1.15x); at K = 1536 and 8192 rows or more the two kernels are even (gemm_bench, H100
+  // 80GB HBM3 at 400 W).  From 512 to 4096 rows the 1-CTA kernel is ahead by a median 1.06x,
+  // about the spread between two runs of the same shape, and 5376 x 640 x 640 is even, so
+  // pairs start once there are enough 128-row tiles to give both CTAs of a cluster work.
   const bool pair = g_gemm_2cta == 1 && a->M >= 512;
   if (a->dtype == DWM_BF16)
     return pair ? dispatch_epi<__nv_bfloat16, __nv_bfloat16, 2>(a, s) : dispatch_epi<__nv_bfloat16, __nv_bfloat16, 1>(a, s);

@@ -1,8 +1,9 @@
-"""Times dwm_b200_linear at the CTSD-3.5 step's GEMM shapes: the 256- and the 128-column tile
-alternately in one process, with torch.matmul (cuBLAS) as a reference.
+"""Times dwm_b200_linear at the CTSD-3.5 step's GEMM shapes: the 256- and the 128-column tile,
+each as the dispatcher runs it (a cluster of two CTAs for M >= 512) and forced to the 1-CTA
+kernel, alternately in one process, with torch.matmul (cuBLAS) as a reference.
 
 Every RESID / GEGLU shape is also run with the plain 16-bit STORE epilogue: the difference
-bounds what the fused epilogue costs.  Both tile widths must give the same bits; the script
+bounds what the fused epilogue costs.  All variants must give the same bits; the script
 checks that on every shape.  The card, its power limit and the median SM clock sampled
 during the timed region are written next to the numbers (bench_out/gemm_bench.json).
 
@@ -31,9 +32,24 @@ SHAPES = [
     (29568, 1536, 1536, "resid"), (29568, 1536, 1536, "store"),
     (29568, 6144, 1536, "store"), (29568, 1536, 6144, "resid"), (29568, 1536, 6144, "store"),
     (8192, 8192, 8192, "store"),
-    # fewer tiles than SMs (either width) and a two-wave middle case, for the tile-width rule
+    # fewer tiles than SMs (either width) and a two-wave middle case, for the tile-width rule;
+    # the pair threshold (M >= 512) from both sides
     (1000, 1536, 1536, "store"), (4096, 1536, 1536, "resid"),
+    (256, 1536, 1536, "store"), (512, 1536, 1536, "store"), (2048, 1536, 1536, "store"),
+    (8192, 1536, 1536, "store"), (16384, 1536, 1536, "store"),
+    # narrow N, where the two widths differ in padding: the CTSD-2.1 UNet's level-1 and
+    # level-2 transformer linears (config 2: 12 items of 32 x 56)
+    (21504, 320, 320, "store"), (21504, 320, 1280, "store"), (5376, 640, 640, "store"),
 ]
+# name -> (option gemm_bn, option gemm_2cta)
+VARIANTS = {"bn256": (256, 1), "bn128": (128, 1), "bn256_1cta": (256, 0), "bn128_1cta": (128, 0)}
+
+
+def select(bn, cta2):
+    lib.set_option("gemm_bn", bn)
+    lib.set_option("gemm_2cta", cta2)
+
+
 def timeit(fn, iters, warm=2):
     for _ in range(warm):
         fn()
@@ -91,26 +107,27 @@ def run_shape(M, N, K, epi, dtype, iters, rounds):
     def call():
         ops.linear(a, w, **kw)
 
-    widths = {"bn256": 256} if epi == "geglu" else {"bn256": 256, "bn128": 128}
-    # same bits from both widths (the blend output is reset: it is also an input)
+    # GEGLU always runs the 256-wide tile
+    variants = {k: v for k, v in VARIANTS.items() if epi != "geglu" or v[0] == 256}
+    # same bits from every variant (the blend output is reset: it is also an input)
     res = {}
-    for name, bn in widths.items():
-        lib.set_option("gemm_bn", bn)
-        if blend:
-            out.copy_(x0)
-        call()
-        res[name] = out.clone()
-    identical = all(torch.equal(r, res["bn256"]) for r in res.values())
-    del res
-    ms = {k: [] for k in list(widths) + ["cublas"]}
     try:
+        for name, (bn, cta2) in variants.items():
+            select(bn, cta2)
+            if blend:
+                out.copy_(x0)
+            call()
+            res[name] = out.clone()
+        identical = all(torch.equal(r, res["bn256"]) for r in res.values())
+        del res
+        ms = {k: [] for k in list(variants) + ["cublas"]}
         for _ in range(rounds):
-            for name, bn in widths.items():
-                lib.set_option("gemm_bn", bn)
+            for name, (bn, cta2) in variants.items():
+                select(bn, cta2)
                 ms[name].append(timeit(call, iters))
             ms["cublas"].append(timeit(lambda: torch.matmul(a, w.t()), iters))
     finally:
-        lib.set_option("gemm_bn", 0)
+        select(0, -1)   # the defaults: tile width by rule, pairs from DWM_GEMM_2CTA
     fl = 2.0 * M * N * K
     row = dict(M=M, N=N, K=K, epi=epi, dtype=str(dtype).split(".")[-1],
                identical_bits=identical)
