@@ -28,6 +28,8 @@ import torch
 from opendwm_b200 import lib as _lib
 from opendwm_b200 import ops as _ops
 
+from .packing import Linear, conv, fp32, gemm, pack_conv, pack_linear, pack_norm
+
 
 class _Cfg(dict):
     __getattr__ = dict.get
@@ -56,6 +58,27 @@ def _attention(channels, groups):
     m.to_v = torch.nn.Linear(channels, channels)
     m.to_out = torch.nn.ModuleList([torch.nn.Linear(channels, channels)])
     return m
+
+
+def _pack_resnet(m, dt, dev):
+    p = dict(n1=pack_norm(m.norm1), c1=pack_conv(m.conv1, dt, dev), n2=pack_norm(m.norm2),
+             c2=pack_conv(m.conv2, dt, dev))
+    if hasattr(m, "conv_shortcut"):
+        p["sc"] = pack_linear(m.conv_shortcut.weight, m.conv_shortcut.bias, dt, dev)
+    return p
+
+
+def _pack_attention(a, dt, dev):
+    """q|k as one Linear, the V projection weight (the A operand of V^T = W_v X^T) and the
+    output Linear with the V bias folded into its bias."""
+    out = pack_linear(a.to_out[0].weight, a.to_out[0].bias, dt, dev)
+    # softmax rows sum to 1: P (V + 1 b_v^T) = P V + b_v^T  =>  fold b_v into b_o
+    bo = out.b + a.to_out[0].weight.detach().float().to(dev) @ fp32(a.to_v.bias.to(dev))
+    return dict(gn=pack_norm(a.group_norm),
+                qk=pack_linear(torch.cat([a.to_q.weight, a.to_k.weight]),
+                               torch.cat([a.to_q.bias, a.to_k.bias]), dt, dev),
+                wv=pack_linear(a.to_v.weight, None, dt, dev).w,
+                out=out._replace(b=bo.contiguous()))
 
 
 class DiagonalGaussianDistribution:
@@ -217,65 +240,32 @@ class AutoencoderKL(torch.nn.Module):
             raise RuntimeError("AutoencoderKL.decode runs on CUDA (sm_90a) only; there "
                                "is no CPU fallback.")
         dt = self.compute_dtype
-
-        def pad8(n):
-            return (n + 7) // 8 * 8
-
-        def conv3(c, pad_in=None, pad_out=None):
-            w = _ops.pack_conv_weight(c.weight.to(dev), dt, pad_out_to=pad_out,
-                                      pad_in_to=pad_in)
-            b = torch.zeros(w.shape[1], device=dev)
-            b[:c.out_channels] = c.bias.detach().float()
-            return w, b
-
-        def lin(weight, bias):
-            return (weight.detach().reshape(weight.shape[0], -1).to(dev, dt).contiguous(),
-                    bias.detach().float().to(dev).contiguous())
-
-        def gn(n):
-            return (n.weight.detach().float().to(dev).contiguous(),
-                    n.bias.detach().float().to(dev).contiguous())
-
-        def res(m):
-            p = dict(n1=gn(m.norm1), c1=conv3(m.conv1), n2=gn(m.norm2), c2=conv3(m.conv2))
-            if hasattr(m, "conv_shortcut"):
-                p["sc"] = lin(m.conv_shortcut.weight, m.conv_shortcut.bias)
-            return p
-
         lc = self.config.latent_channels
+        cp = (lc + 7) // 8 * 8
         if hasattr(self, "post_quant_conv"):
             # 1x1 conv as a GEMM whose N is padded to the 32-column tile granule; conv_in
             # then reads those 32 (zero-extended) channels
             cq = (lc + 31) // 32 * 32
-            w = torch.zeros(cq, pad8(lc), device=dev, dtype=dt)
+            w = torch.zeros(cq, cp, device=dev, dtype=dt)
             w[:lc, :lc] = self.post_quant_conv.weight.detach().reshape(lc, lc).to(dev, dt)
             b = torch.zeros(cq, device=dev)
             b[:lc] = self.post_quant_conv.bias.detach().float()
-            pk = dict(pq=(w, b), conv_in=conv3(d.conv_in, pad_in=cq))
+            pk = dict(pq=Linear(w, b), conv_in=pack_conv(d.conv_in, dt, dev, pad_in=cq))
         else:
-            pk = dict(conv_in=conv3(d.conv_in, pad_in=pad8(lc)))
-        pk["mid"] = [res(r) for r in d.mid_block.resnets]
+            pk = dict(conv_in=pack_conv(d.conv_in, dt, dev, pad_in=cp))
+        pk["mid"] = [_pack_resnet(r, dt, dev) for r in d.mid_block.resnets]
         pk["attn"] = None
         if len(d.mid_block.attentions):
-            a = d.mid_block.attentions[0]
-            wq, bq = lin(a.to_q.weight, a.to_q.bias)
-            wk, bk = lin(a.to_k.weight, a.to_k.bias)
-            wv, bv = lin(a.to_v.weight, a.to_v.bias)
-            wo, bo = lin(a.to_out[0].weight, a.to_out[0].bias)
-            # softmax rows sum to 1: P (V + 1 b_v^T) = P V + b_v^T  =>  fold b_v into b_o
-            bo = bo + a.to_out[0].weight.detach().float().to(dev) @ bv
-            pk["attn"] = dict(gn=gn(a.group_norm), wqk=torch.cat([wq, wk]).contiguous(),
-                              bqk=torch.cat([bq, bk]).contiguous(), wv=wv, wo=wo,
-                              bo=bo.contiguous())
+            pk["attn"] = _pack_attention(d.mid_block.attentions[0], dt, dev)
         pk["ups"] = []
         for blk in d.up_blocks:
-            b = dict(res=[res(r) for r in blk.resnets])
+            b = dict(res=[_pack_resnet(r, dt, dev) for r in blk.resnets])
             if hasattr(blk, "upsamplers"):
-                b["up"] = conv3(blk.upsamplers[0].conv)
+                b["up"] = pack_conv(blk.upsamplers[0].conv, dt, dev)
             pk["ups"].append(b)
-        pk["norm_out"] = gn(d.conv_norm_out)
+        pk["norm_out"] = pack_norm(d.conv_norm_out)
         co = self.config.out_channels
-        pk["conv_out"] = conv3(d.conv_out, pad_out=(co + 31) // 32 * 32)
+        pk["conv_out"] = pack_conv(d.conv_out, dt, dev, pad_out=(co + 31) // 32 * 32)
         self._pk = pk
         return pk
 
@@ -288,20 +278,20 @@ class AutoencoderKL(torch.nn.Module):
         groups = self.config.norm_num_groups
         sums = _ops.groupnorm_stats(h5, groups)
         out = torch.empty(nb, 1, H, W, C, device=h.device, dtype=self.compute_dtype)
-        _ops.spatialnorm_silu(h5, sums, p[0], p[1], out, groups=groups, eps=1e-6, silu=silu)
+        _ops.spatialnorm_silu(h5, sums, p[0], p[1], out, groups=groups, eps=p[2], silu=silu)
         return out
 
     def _resnet(self, h, shape, p):
         a = self._norm(h, shape, p["n1"], True)
-        h1 = _ops.conv(a, *p["c1"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+        h1 = conv(a, p["c1"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         b = self._norm(h1, shape, p["n2"], True)
         if "sc" in p:
             h16 = torch.empty(h.shape, device=h.device, dtype=self.compute_dtype)
             _ops.act_cast(h, h16)
-            skip = _ops.linear(h16, *p["sc"], epilogue=_lib.EPI_F32)
+            skip = gemm(h16, p["sc"], epilogue=_lib.EPI_F32)
         else:
             skip = h
-        return _ops.conv(b, *p["c2"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID, resid=skip)
+        return conv(b, p["c2"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID, resid=skip)
 
     def _attn(self, h, shape, p):
         nb, H, W = shape
@@ -311,7 +301,7 @@ class AutoencoderKL(torch.nn.Module):
                              "resolution (16-byte TMA pitch); got {}x{}".format(H, W))
         dt = self.compute_dtype
         xn = self._norm(h, shape, p["gn"], False).view(nb * HW, C)
-        qk = _ops.linear(xn, p["wqk"], p["bqk"])                     # [P, 2C] 16-bit
+        qk = gemm(xn, p["qk"])                                      # [P, 2C] 16-bit
         vt = _ops.linear(p["wv"], xn)                               # V^T [C, P]
         o = torch.empty(nb * HW, C, device=h.device, dtype=dt)
         s = torch.empty(HW, HW, device=h.device, dtype=torch.float32)
@@ -322,7 +312,7 @@ class AutoencoderKL(torch.nn.Module):
             _ops.linear(qk[r, :C], qk[r, C:], epilogue=_lib.EPI_F32, out=s)
             _ops.softmax_rows(s, scale, pr)
             _ops.linear(pr, vt[:, r], out=o[r])
-        return _ops.linear(o, p["wo"], p["bo"], epilogue=_lib.EPI_RESID, resid=h)
+        return gemm(o, p["out"], epilogue=_lib.EPI_RESID, resid=h)
 
     # -- encoder ---------------------------------------------------------------------------------
     @torch.no_grad()
@@ -334,54 +324,27 @@ class AutoencoderKL(torch.nn.Module):
             raise RuntimeError("AutoencoderKL.encode runs on CUDA (sm_90a) only; there is no "
                                "CPU fallback.")
         dt = self.compute_dtype
-
-        def conv3(c, pad_in=None, pad_out=None):
-            w = _ops.pack_conv_weight(c.weight.to(dev), dt, pad_out_to=pad_out, pad_in_to=pad_in)
-            b = torch.zeros(w.shape[1], device=dev)
-            b[:c.out_channels] = c.bias.detach().float()
-            return w, b
-
-        def lin(weight, bias):
-            return (weight.detach().reshape(weight.shape[0], -1).to(dev, dt).contiguous(),
-                    bias.detach().float().to(dev).contiguous())
-
-        def gn(n):
-            return (n.weight.detach().float().to(dev).contiguous(),
-                    n.bias.detach().float().to(dev).contiguous())
-
-        def res(m):
-            p = dict(n1=gn(m.norm1), c1=conv3(m.conv1), n2=gn(m.norm2), c2=conv3(m.conv2))
-            if hasattr(m, "conv_shortcut"):
-                p["sc"] = lin(m.conv_shortcut.weight, m.conv_shortcut.bias)
-            return p
-        pk = dict(conv_in=conv3(e.conv_in, pad_in=16), downs=[])   # 16 = smallest validated C_in
+        # 16 = smallest validated C_in
+        pk = dict(conv_in=pack_conv(e.conv_in, dt, dev, pad_in=16), downs=[])
         for blk in e.down_blocks:
-            b = dict(res=[res(r) for r in blk.resnets])
+            b = dict(res=[_pack_resnet(r, dt, dev) for r in blk.resnets])
             if hasattr(blk, "downsamplers"):
-                b["down"] = conv3(blk.downsamplers[0].conv)
+                b["down"] = pack_conv(blk.downsamplers[0].conv, dt, dev)
             pk["downs"].append(b)
-        pk["mid"] = [res(r) for r in e.mid_block.resnets]
+        pk["mid"] = [_pack_resnet(r, dt, dev) for r in e.mid_block.resnets]
         pk["attn"] = None
         if len(e.mid_block.attentions):
-            a = e.mid_block.attentions[0]
-            wq, bq = lin(a.to_q.weight, a.to_q.bias)
-            wk, bk = lin(a.to_k.weight, a.to_k.bias)
-            wv, bv = lin(a.to_v.weight, a.to_v.bias)
-            wo, bo = lin(a.to_out[0].weight, a.to_out[0].bias)
-            bo = bo + a.to_out[0].weight.detach().float().to(dev) @ bv
-            pk["attn"] = dict(gn=gn(a.group_norm), wqk=torch.cat([wq, wk]).contiguous(),
-                              bqk=torch.cat([bq, bk]).contiguous(), wv=wv, wo=wo,
-                              bo=bo.contiguous())
-        pk["norm_out"] = gn(e.conv_norm_out)
+            pk["attn"] = _pack_attention(e.mid_block.attentions[0], dt, dev)
+        pk["norm_out"] = pack_norm(e.conv_norm_out)
         lc2 = 2 * self.config.latent_channels
         cq = (lc2 + 31) // 32 * 32
-        pk["conv_out"] = conv3(e.conv_out, pad_out=cq)
+        pk["conv_out"] = pack_conv(e.conv_out, dt, dev, pad_out=cq)
         if hasattr(self, "quant_conv"):
             w = torch.zeros(cq, cq, device=dev, dtype=dt)
             w[:lc2, :lc2] = self.quant_conv.weight.detach().reshape(lc2, lc2).to(dev, dt)
             b = torch.zeros(cq, device=dev)
             b[:lc2] = self.quant_conv.bias.detach().float()
-            pk["quant"] = (w, b)
+            pk["quant"] = Linear(w, b)
         self._pk_enc = pk
         return pk
 
@@ -399,9 +362,9 @@ class AutoencoderKL(torch.nn.Module):
         nb, cin, H, W = x.shape
         if H % 2 ** (len(pk["downs"]) - 1) or W % 2 ** (len(pk["downs"]) - 1):
             raise ValueError("image size must be divisible by the VAE down-sampling factor")
-        x16 = torch.zeros(nb, 1, H, W, pk["conv_in"][0].shape[2], device=x.device, dtype=dt)
+        x16 = torch.zeros(nb, 1, H, W, pk["conv_in"].w.shape[2], device=x.device, dtype=dt)
         x16[..., :cin] = x.permute(0, 2, 3, 1).unsqueeze(1)
-        h = _ops.conv(x16, *pk["conv_in"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+        h = conv(x16, pk["conv_in"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         shape = (nb, H, W)
         for blk in pk["downs"]:
             for p in blk["res"]:
@@ -410,8 +373,8 @@ class AutoencoderKL(torch.nn.Module):
                 n, H, W = shape
                 h16 = torch.empty(h.shape, device=h.device, dtype=dt)
                 _ops.act_cast(h, h16)
-                y = _ops.conv(h16.view(n, 1, H, W, -1), *blk["down"], kernel=(1, 3, 3),
-                              epilogue=_lib.EPI_F32)
+                y = conv(h16.view(n, 1, H, W, -1), blk["down"], kernel=(1, 3, 3),
+                         epilogue=_lib.EPI_F32)
                 C = y.shape[1]
                 h = y.view(n, H, W, C)[:, 1::2, 1::2].contiguous().view(-1, C)
                 shape = (n, H // 2, W // 2)
@@ -421,10 +384,10 @@ class AutoencoderKL(torch.nn.Module):
         h = self._resnet(h, shape, pk["mid"][1])
         a = self._norm(h, shape, pk["norm_out"], True)
         if "quant" in pk:
-            m16 = _ops.conv(a, *pk["conv_out"], kernel=(1, 3, 3), epilogue=_lib.EPI_STORE)
-            moments = _ops.linear(m16, *pk["quant"], epilogue=_lib.EPI_F32)
+            m16 = conv(a, pk["conv_out"], kernel=(1, 3, 3), epilogue=_lib.EPI_STORE)
+            moments = gemm(m16, pk["quant"], epilogue=_lib.EPI_F32)
         else:
-            moments = _ops.conv(a, *pk["conv_out"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+            moments = conv(a, pk["conv_out"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         n, H, W = shape
         lc = self.config.latent_channels
         moments = moments.view(n, H, W, -1)[..., :2 * lc].permute(0, 3, 1, 2).contiguous()
@@ -444,12 +407,12 @@ class AutoencoderKL(torch.nn.Module):
             self._pack()
         pk, dt = self._pk, self.compute_dtype
         nb, lc, H, W = z.shape
-        cp = pk["pq"][0].shape[1] if "pq" in pk else pk["conv_in"][0].shape[2]
+        cp = pk["pq"].w.shape[1] if "pq" in pk else pk["conv_in"].w.shape[2]
         x16 = torch.zeros(nb, 1, H, W, cp, device=z.device, dtype=dt)
         x16[..., :lc] = z.permute(0, 2, 3, 1).unsqueeze(1)
         if "pq" in pk:
-            x16 = _ops.linear(x16.view(-1, cp), *pk["pq"]).view(nb, 1, H, W, -1)
-        h = _ops.conv(x16, *pk["conv_in"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+            x16 = gemm(x16.view(-1, cp), pk["pq"]).view(nb, 1, H, W, -1)
+        h = conv(x16, pk["conv_in"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         shape = (nb, H, W)
         h = self._resnet(h, shape, pk["mid"][0])
         if pk["attn"] is not None:
@@ -462,9 +425,9 @@ class AutoencoderKL(torch.nn.Module):
                 n, H, W = shape
                 u = _ops.upsample_nearest(h.view(n, 1, H, W, -1), False, dt)
                 shape = (n, 2 * H, 2 * W)
-                h = _ops.conv(u, *blk["up"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+                h = conv(u, blk["up"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         a = self._norm(h, shape, pk["norm_out"], True)
-        y = _ops.conv(a, *pk["conv_out"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+        y = conv(a, pk["conv_out"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         n, H, W = shape
         dec = y.view(n, H, W, -1)[..., :self.config.out_channels]\
             .permute(0, 3, 1, 2).contiguous().to(z.dtype)

@@ -29,6 +29,8 @@ import torch
 from opendwm_b200 import lib as _lib
 from opendwm_b200 import ops as _ops
 
+from .packing import conv, gemm, pack_conv, pack_linear, pack_norm
+
 
 class _Cfg(dict):
     __getattr__ = dict.get
@@ -50,6 +52,13 @@ def _spatial_norm(f, zq, groups):
     m.conv_y = _causal(zq, f, 1)
     m.conv_b = _causal(zq, f, 1)
     return m
+
+
+def _pack_spatial_norm(m, dt, dev):
+    """GroupNorm triple and the conv_y / conv_b (1x1x1) Linears of a SpatialNorm3D."""
+    return dict(norm=pack_norm(m.norm_layer),
+                y=pack_linear(m.conv_y.conv.weight, m.conv_y.conv.bias, dt, dev),
+                b=pack_linear(m.conv_b.conv.weight, m.conv_b.conv.bias, dt, dev))
 
 
 def _resnet(cin, cout, zq, groups):
@@ -201,49 +210,29 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
                                "only; there is no CPU fallback.")
         dt = self.compute_dtype
 
-        def conv3(m, pad_out=None):
-            w = _ops.pack_conv_weight(m.conv.weight.to(dev), dt, pad_out_to=pad_out)
-            b = m.conv.bias.detach().float().to(dev)
-            if pad_out and pad_out != b.numel():
-                bp = torch.zeros(pad_out, device=dev)
-                bp[:b.numel()] = b
-                b = bp
-            return w, b.contiguous()
-
-        def lin(conv):      # 1x1x1 conv -> [C_out, C_in] GEMM weight
-            w = conv.weight.detach().reshape(conv.out_channels, -1).to(dev, dt)
-            return w.contiguous(), conv.bias.detach().float().to(dev).contiguous()
-
-        def sn(m):
-            return dict(gamma=m.norm_layer.weight.detach().float().to(dev).contiguous(),
-                        beta=m.norm_layer.bias.detach().float().to(dev).contiguous(),
-                        y=lin(m.conv_y.conv), b=lin(m.conv_b.conv))
-
         def res(m):
-            p = dict(n1=sn(m.norm1), c1=conv3(m.conv1), n2=sn(m.norm2),
-                     c2=conv3(m.conv2))
+            p = dict(n1=_pack_spatial_norm(m.norm1, dt, dev), c1=pack_conv(m.conv1.conv, dt, dev),
+                     n2=_pack_spatial_norm(m.norm2, dt, dev), c2=pack_conv(m.conv2.conv, dt, dev))
             if hasattr(m, "conv_shortcut"):
-                p["sc"] = lin(m.conv_shortcut)
+                p["sc"] = pack_linear(m.conv_shortcut.weight, m.conv_shortcut.bias, dt, dev)
             return p
 
         d = self.decoder
-        pk = dict(conv_in=conv3(d.conv_in),
+        pk = dict(conv_in=pack_conv(d.conv_in.conv, dt, dev),
                   mid=[res(r) for r in d.mid_block.resnets], ups=[])
         for blk in d.up_blocks:
             b = dict(res=[res(r) for r in blk.resnets], compress=blk.compress_time)
             if hasattr(blk, "upsamplers"):
-                c = blk.upsamplers[0].conv
-                b["up"] = (_ops.pack_conv_weight(c.weight.to(dev), dt),
-                           c.bias.detach().float().to(dev).contiguous())
+                b["up"] = pack_conv(blk.upsamplers[0].conv, dt, dev)
             pk["ups"].append(b)
-        pk["norm_out"] = sn(d.norm_out)
+        pk["norm_out"] = _pack_spatial_norm(d.norm_out, dt, dev)
         cout = self.config.out_channels
-        pk["conv_out"] = conv3(d.conv_out, pad_out=32 if cout < 32 else None)
+        pk["conv_out"] = pack_conv(d.conv_out.conv, dt, dev, pad_out=32 if cout < 32 else None)
         self._pk = pk
         return pk
 
     # -- building blocks ---------------------------------------------------------------------
-    def _causal_conv(self, name, x_pad, wb, cache, new_cache, **kw):
+    def _causal_conv(self, name, x_pad, c, cache, new_cache, **kw):
         """x_pad: 16-bit [nb, T+2, H, W, C] whose frames [2:] are filled; the two leading
         frames become the cached tail of the previous chunk or replicas of frame 0."""
         prev = cache.get(name)
@@ -255,7 +244,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         # that nothing writes again), copied once into the next chunk's padding: one copy per
         # convolution and chunk instead of clone + copy
         new_cache[name] = x_pad[:, -2:]
-        return _ops.conv(x_pad, wb[0], wb[1], kernel=(3, 3, 3), **kw)
+        return conv(x_pad, c, kernel=(3, 3, 3), **kw)
 
     def _norm_act(self, h, shape, p, zq16, zshape, groups):
         """SpatialNorm3D + SiLU of fp32 `h` [rows, C] -> 16-bit time-padded conv input."""
@@ -263,11 +252,12 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         C = h.shape[1]
         h5 = h.view(nb, T, H, W, C)
         sums = _ops.groupnorm_stats(h5, groups)
-        zy = _ops.linear(zq16, *p["y"], epilogue=_lib.EPI_F32).view(*zshape, C)
-        zb = _ops.linear(zq16, *p["b"], epilogue=_lib.EPI_F32).view(*zshape, C)
+        zy = gemm(zq16, p["y"], epilogue=_lib.EPI_F32).view(*zshape, C)
+        zb = gemm(zq16, p["b"], epilogue=_lib.EPI_F32).view(*zshape, C)
         out = torch.empty(nb, T + 2, H, W, C, device=h.device, dtype=self.compute_dtype)
-        _ops.spatialnorm_silu(h5, sums, p["gamma"], p["beta"], out, groups=groups,
-                              eps=1e-6, zy=zy, zb=zb, out_t0=2, silu=True)
+        g = p["norm"]
+        _ops.spatialnorm_silu(h5, sums, g[0], g[1], out, groups=groups,
+                              eps=g[2], zy=zy, zb=zb, out_t0=2, silu=True)
         return out
 
     def _resnet(self, name, h, shape, p, zq16, zshape, groups, cache, new_cache):
@@ -278,7 +268,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         if "sc" in p:
             h16 = torch.empty(h.shape, device=h.device, dtype=self.compute_dtype)
             _ops.act_cast(h, h16)
-            skip = _ops.linear(h16, *p["sc"], epilogue=_lib.EPI_F32)
+            skip = gemm(h16, p["sc"], epilogue=_lib.EPI_F32)
         else:
             skip = h
         return self._causal_conv(name + ".conv2", b, p["c2"], cache, new_cache,
@@ -309,8 +299,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
                 n, T, H, W = shape
                 u = _ops.upsample_nearest(h.view(n, T, H, W, -1), blk["compress"], dt)
                 shape = (n, u.shape[1], 2 * H, 2 * W)
-                h = _ops.conv(u, blk["up"][0], blk["up"][1], kernel=(1, 3, 3),
-                              epilogue=_lib.EPI_F32)
+                h = conv(u, blk["up"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         a = self._norm_act(h, shape, pk["norm_out"], zq16, zshape, groups)
         y = self._causal_conv("conv_out", a, pk["conv_out"], cache, new_cache,
                               epilogue=_lib.EPI_F32)
@@ -327,35 +316,22 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
                                "there is no CPU fallback.")
         dt = self.compute_dtype
 
-        def conv3(conv, pad_in=None, pad_out=None):
-            w = _ops.pack_conv_weight(conv.weight.to(dev), dt, pad_out_to=pad_out,
-                                      pad_in_to=pad_in)
-            b = torch.zeros(w.shape[1], device=dev)
-            b[:conv.out_channels] = conv.bias.detach().float()
-            return w, b
-
-        def gn(n):
-            return (n.weight.detach().float().to(dev).contiguous(),
-                    n.bias.detach().float().to(dev).contiguous())
-
         def res(m):
-            p = dict(n1=gn(m.norm1), c1=conv3(m.conv1.conv), n2=gn(m.norm2),
-                     c2=conv3(m.conv2.conv))
+            p = dict(n1=pack_norm(m.norm1), c1=pack_conv(m.conv1.conv, dt, dev),
+                     n2=pack_norm(m.norm2), c2=pack_conv(m.conv2.conv, dt, dev))
             if hasattr(m, "conv_shortcut"):
-                c = m.conv_shortcut
-                p["sc"] = (c.weight.detach().reshape(c.out_channels, -1).to(dev, dt).contiguous(),
-                           c.bias.detach().float().to(dev).contiguous())
+                p["sc"] = pack_linear(m.conv_shortcut.weight, m.conv_shortcut.bias, dt, dev)
             return p
-        pk = dict(conv_in=conv3(e.conv_in.conv, pad_in=16), downs=[])
+        pk = dict(conv_in=pack_conv(e.conv_in.conv, dt, dev, pad_in=16), downs=[])
         for blk in e.down_blocks:
             b = dict(res=[res(r) for r in blk.resnets], compress=blk.compress_time)
             if hasattr(blk, "downsamplers"):
-                b["down"] = conv3(blk.downsamplers[0].conv)
+                b["down"] = pack_conv(blk.downsamplers[0].conv, dt, dev)
             pk["downs"].append(b)
         pk["mid"] = [res(r) for r in e.mid_block.resnets]
-        pk["norm_out"] = gn(e.norm_out)
+        pk["norm_out"] = pack_norm(e.norm_out)
         lc2 = 2 * self.config.latent_channels
-        pk["conv_out"] = conv3(e.conv_out.conv, pad_out=(lc2 + 31) // 32 * 32)
+        pk["conv_out"] = pack_conv(e.conv_out.conv, dt, dev, pad_out=(lc2 + 31) // 32 * 32)
         self._pk_enc = pk
         return pk
 
@@ -366,7 +342,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         h5 = h.view(nb, T, H, W, C)
         sums = _ops.groupnorm_stats(h5, groups)
         out = torch.empty(nb, T + 2, H, W, C, device=h.device, dtype=self.compute_dtype)
-        _ops.spatialnorm_silu(h5, sums, p[0], p[1], out, groups=groups, eps=1e-6, out_t0=2,
+        _ops.spatialnorm_silu(h5, sums, p[0], p[1], out, groups=groups, eps=p[2], out_t0=2,
                               silu=True)
         return out
 
@@ -378,7 +354,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         if "sc" in p:
             h16 = torch.empty(h.shape, device=h.device, dtype=self.compute_dtype)
             _ops.act_cast(h, h16)
-            skip = _ops.linear(h16, *p["sc"], epilogue=_lib.EPI_F32)
+            skip = gemm(h16, p["sc"], epilogue=_lib.EPI_F32)
         else:
             skip = h
         return self._causal_conv(name + ".conv2", b, p["c2"], cache, new_cache,
@@ -405,7 +381,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
             T = h5.shape[1]
         x16 = torch.empty(nb, T, H, W, C, device=h.device, dtype=self.compute_dtype)
         _ops.act_cast(h5.contiguous(), x16)
-        y = _ops.conv(x16, *blk["down"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+        y = conv(x16, blk["down"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         y = y.view(nb, T, H, W, C)[:, :, 1::2, 1::2].contiguous()
         return y.view(-1, C), (nb, T, H // 2, W // 2)
 
@@ -415,7 +391,7 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         groups = self.config.norm_num_groups
         nb, T, H, W, cin = x.shape
         new_cache = {}
-        cp = pk["conv_in"][0].shape[2]
+        cp = pk["conv_in"].w.shape[2]
         xin = torch.zeros(nb, T + 2, H, W, cp, device=x.device, dtype=dt)
         xin[:, 2:, ..., :cin] = x
         h = self._causal_conv("enc.conv_in", xin, pk["conv_in"], cache, new_cache,

@@ -11,30 +11,11 @@ import torch
 from opendwm_b200 import lib as _lib
 from opendwm_b200 import ops as _ops
 
+from .packing import fp32, gemm, layernorm, pack_linear, pack_norm, requantize
+
 
 class ParamGroup(torch.nn.Module):
     """Pure namespace: gives nested parameters the reference's dotted key names."""
-
-
-def gemm(a, w, **kw):
-    """Runs one packed linear.  16-bit: `a` is the operand, w = (weight, bias).  FP8:
-    a = (E4M3 operand, row scales), w = (E4M3 weight, bias, channel scales, 16-bit output
-    dtype)."""
-    if len(w) == 2:
-        return _ops.linear(a, w[0], w[1], **kw)
-    return _ops.linear(a[0], w[0], w[1], a_scale=a[1], w_scale=w[2], out_dtype=w[3], **kw)
-
-
-def fp8_operand(ws, key, t):
-    """E4M3 copy (with row scales) of the 16-bit GEMM operand t in the workspace buffers
-    ws[key], ws[key + "_s"]; returns it in the form `gemm` takes."""
-    return _ops.quantize_rows(t, ws[key][:t.shape[0], :t.shape[1]], ws[key + "_s"][:t.shape[0]])
-
-
-def packed(p, name):
-    """The `gemm` weight tuple of linear `name` of a VTSelfAttentionBlock pack."""
-    w = (p[name + "_w"], p[name + "_b"])
-    return w + (p[name + "_s"], p["out_dtype"]) if p.get("fp8") else w
 
 
 def make_feed_forward(dim, dim_out=None, mult=4, activation_fn="geglu"):
@@ -156,50 +137,28 @@ class VTSelfAttentionBlock(torch.nn.Module):
         self._packed = None
 
     def pack(self, dtype, device, fp8=False):
-        """Packs the weights for `run`.  fp8: every linear is stored as E4M3 with one fp32
-        scale per output channel (key suffix _s), quantized from the parameters' own
-        precision; 16-bit outputs stay `dtype`."""
-        p = {"fp8": fp8, "out_dtype": dtype, "fp8_bytes_saved": 0}
-
-        def w16(t):
-            return t.detach().to(device=device, dtype=dtype).contiguous()
-
-        def f32(t):
-            return None if t is None else \
-                t.detach().to(device=device, dtype=torch.float32).contiguous()
-
-        def put(name, w, b):
-            if fp8:
-                p[name + "_w"], p[name + "_s"] = _ops.quantize_weight_rows(w.to(device))
-                p["fp8_bytes_saved"] += w.numel() * (dtype.itemsize - 1) - 4 * w.shape[0]
-            else:
-                p[name + "_w"] = w16(w)
-            p[name + "_b"] = f32(b)
-
+        """Packs the weights for `run`: a dict of `Linear`s (ff_in1, ff_in2, qkv, out, ff1,
+        ff2) and LayerNorm triples.  fp8: every linear is E4M3 with one fp32 scale per output
+        channel, quantized from the parameters' own precision; 16-bit outputs stay `dtype`."""
+        p = {}
         for name, ff in (("ff_in", self.ff_in), ("ff", self.ff)):
             w, b = _ops.pack_geglu(
                 ff.net[0].proj.weight.detach().to(device),
                 ff.net[0].proj.bias.detach().to(device))
-            put(name + "1", w, b)       # FP8: quantized after packing, scales follow rows
-            put(name + "2", ff.net[2].weight, ff.net[2].bias)
+            # FP8: quantized after the GEGLU row packing, scales follow the rows
+            p[name + "1"] = pack_linear(w, b, dtype, device, fp8)
+            p[name + "2"] = pack_linear(ff.net[2].weight, ff.net[2].bias, dtype, device, fp8)
         at = self.attn1
-        put("qkv", torch.cat([at.to_q.weight, at.to_k.weight, at.to_v.weight]),
+        p["qkv"] = pack_linear(
+            torch.cat([at.to_q.weight, at.to_k.weight, at.to_v.weight]),
             None if at.to_q.bias is None else
-            torch.cat([at.to_q.bias, at.to_k.bias, at.to_v.bias]))
-        D = self.dim
-        p["q_w"], p["kv_w"] = p["qkv_w"][:D], p["qkv_w"][D:]   # row slices (views)
-        p["q_b"] = None if p["qkv_b"] is None else p["qkv_b"][:D]
-        p["kv_b"] = None if p["qkv_b"] is None else p["qkv_b"][D:]
-        if fp8:
-            p["q_s"], p["kv_s"] = p["qkv_s"][:D], p["qkv_s"][D:]
+            torch.cat([at.to_q.bias, at.to_k.bias, at.to_v.bias]), dtype, device, fp8)
         p["qk_norm"] = at.qk_norm == "rms_norm"
         if p["qk_norm"]:
-            p["nq"], p["nk"] = f32(at.norm_q.weight), f32(at.norm_k.weight)
-        put("out", at.to_out[0].weight, at.to_out[0].bias)
+            p["nq"], p["nk"] = fp32(at.norm_q.weight), fp32(at.norm_k.weight)
+        p["out"] = pack_linear(at.to_out[0].weight, at.to_out[0].bias, dtype, device, fp8)
         for n in ("norm_in", "norm1", "norm3"):
-            m = getattr(self, n)
-            p[n + "_w"], p[n + "_b"], p[n + "_eps"] = \
-                f32(m.weight), f32(m.bias), m.eps
+            p[n] = pack_norm(getattr(self, n))
         self._packed = p
         return p
 
@@ -208,42 +167,31 @@ class VTSelfAttentionBlock(torch.nn.Module):
         """x: fp32 residual stream [M, D] (updated in place with the blended result);
         emb: fp32 [items, D] added before the block (view / frame index embedding);
         attend(qkv, out): launches the regrouped attention; alpha: fp32 [B];
-        qkv_attend(p, a16, out): optional replacement of projection + attention
-        (frame-sharded temporal attention with a K,V all-gather; it receives the operand
-        in the form `gemm` takes).  FP8 packs: the LayerNorms write E4M3 operands with row
-        scales, the GEGLU and attention outputs are quantized before their projections."""
+        qkv_attend(p, a, out): optional replacement of projection + attention
+        (frame-sharded temporal attention with a K,V all-gather; it receives the LayerNorm
+        output Operand).  ws["a"] is the LayerNorm output Operand and ws["q"] the E4M3 buffer
+        the GEGLU and attention outputs are requantized into (None in 16 bit)."""
         D = self.dim
-        y, g16, qkv, o16 = ws["y"], ws["g16"], ws["qkv_s"], ws["o16"]
-        fp8 = p.get("fp8", False)
-        a = (ws["a8"], ws["a8_s"]) if fp8 else ws["a16"]
-
-        def ln(src, **kw):
-            if fp8:
-                _ops.layernorm(src, a[0], out_scale=a[1], **kw)
-            else:
-                _ops.layernorm(src, a, **kw)
-
-        def operand(t):    # the 16-bit GEMM output t as the next GEMM's operand
-            return fp8_operand(ws, "q8", t) if fp8 else t
-
-        ln(x, weight=p["norm_in_w"], bias=p["norm_in_b"], eps=p["norm_in_eps"],
-           add_item=emb, rows_per_item=rows_per_item, sum_out=y)
-        gemm(a, packed(p, "ff_in1"), epilogue=_lib.EPI_GEGLU, out=g16)
-        gemm(operand(g16), packed(p, "ff_in2"), epilogue=_lib.EPI_RESID, resid=y, out=y)
-        ln(y, weight=p["norm1_w"], bias=p["norm1_b"], eps=p["norm1_eps"])
+        y, g16, qkv, o16, a, q = ws["y"], ws["g16"], ws["qkv_s"], ws["o16"], ws["a"], ws["q"]
+        n_in, n1, n3 = p["norm_in"], p["norm1"], p["norm3"]
+        layernorm(x, a, weight=n_in[0], bias=n_in[1], eps=n_in[2],
+                  add_item=emb, rows_per_item=rows_per_item, sum_out=y)
+        gemm(a, p["ff_in1"], epilogue=_lib.EPI_GEGLU, out=g16)
+        gemm(requantize(g16, q), p["ff_in2"], epilogue=_lib.EPI_RESID, resid=y, out=y)
+        layernorm(y, a, weight=n1[0], bias=n1[1], eps=n1[2])
         if qkv_attend is not None:
             qkv_attend(p, a, o16)
         else:
             if p["qk_norm"]:
-                gemm(a, packed(p, "qkv"), epilogue=_lib.EPI_QKNORM, out=qkv,
+                gemm(a, p["qkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
                      q_norm_weight=p["nq"], k_norm_weight=p["nk"], qk_region=D,
                      eps=self.attn1.eps)
             else:
-                gemm(a, packed(p, "qkv"), out=qkv)
+                gemm(a, p["qkv"], out=qkv)
             attend(qkv, o16)
-        gemm(operand(o16), packed(p, "out"), epilogue=_lib.EPI_RESID, resid=y, out=y)
-        ln(y, weight=p["norm3_w"], bias=p["norm3_b"], eps=p["norm3_eps"])
-        gemm(a, packed(p, "ff1"), epilogue=_lib.EPI_GEGLU, out=g16)
+        gemm(requantize(o16, q), p["out"], epilogue=_lib.EPI_RESID, resid=y, out=y)
+        layernorm(y, a, weight=n3[0], bias=n3[1], eps=n3[2])
+        gemm(a, p["ff1"], epilogue=_lib.EPI_GEGLU, out=g16)
         # last GEMM: + residual, then AlphaBlender against the un-grafted stream
-        gemm(operand(g16), packed(p, "ff2"), epilogue=_lib.EPI_RESID, resid=y, out=x,
+        gemm(requantize(g16, q), p["ff2"], epilogue=_lib.EPI_RESID, resid=y, out=x,
              blend_x=x, alpha=alpha, rows_per_batch=rows_per_batch)

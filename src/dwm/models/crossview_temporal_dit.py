@@ -31,8 +31,9 @@ from opendwm_b200 import ops as _ops
 from .. import _compat
 from . import adapters as _adapters
 from .crossview_temporal import (
-    AlphaBlender, ParamGroup, VTSelfAttentionBlock, fp8_operand, gemm, make_attention,
-    make_feed_forward, packed)
+    AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward)
+from .packing import (
+    FP8, Operand, fp32, fp8_bytes_saved, gemm, layernorm, pack_linear, requantize)
 
 
 def _sincos_2d(embed_dim, grid_size, base_size, device):
@@ -280,38 +281,16 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
                 "there is no CPU fallback. Move the model to the GPU first.")
         dt = self._dtype()
         D = self.inner_dim
-
-        def w16(t):
-            return t.detach().to(device=dev, dtype=dt).contiguous()
-
-        def f32(t):
-            return t.detach().to(device=dev, dtype=torch.float32).contiguous()
-
-        def lin(m):
-            return w16(m.weight), (None if m.bias is None else f32(m.bias))
-
         fp8 = self.gemm_dtype is not None
-        pk = {"dtype": dt, "fp8": fp8, "fp8_bytes_saved": 0}
-
-        def blk_lin(w, b):
-            """A linear of a joint block: 16-bit, or E4M3 with per-channel scales."""
-            if not fp8:
-                return w16(w), (None if b is None else f32(b))
-            w8, s = _ops.quantize_weight_rows(w.to(dev))
-            pk["fp8_bytes_saved"] += w.numel() * (dt.itemsize - 1) - 4 * w.shape[0]
-            return w8, (None if b is None else f32(b)), s, dt
-
-        def blin(m):
-            return blk_lin(m.weight, m.bias)
-        pe = self.pos_embed.proj
-        pk["patch_w"] = w16(pe.weight.reshape(D, -1))
-        pk["patch_b"] = f32(pe.bias)
+        pk = {"dtype": dt, "fp8": fp8}
+        # 16-bit in either precision: the embedders, the AdaLN linears and proj_out; E4M3
+        # with fp8: the linears of the joint and cross-view / temporal blocks
         te = self.time_text_embed
-        pk["t1"], pk["t2"] = lin(te.timestep_embedder.linear_1), \
-            lin(te.timestep_embedder.linear_2)
-        pk["p1"], pk["p2"] = lin(te.text_embedder.linear_1), \
-            lin(te.text_embedder.linear_2)
-        pk["ctx"] = lin(self.context_embedder)
+        pk["patch"], pk["t1"], pk["t2"], pk["p1"], pk["p2"], pk["ctx"] = (
+            pack_linear(m.weight, m.bias, dt, dev) for m in (
+                self.pos_embed.proj, te.timestep_embedder.linear_1,
+                te.timestep_embedder.linear_2, te.text_embedder.linear_1,
+                te.text_embedder.linear_2, self.context_embedder))
 
         # all AdaLN linears act on the same SiLU(temb): one concatenated GEMM
         mod_w, mod_b, off = [], [], 0
@@ -325,57 +304,57 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
                 b[key] = (off, m.weight.shape[0])
                 off += m.weight.shape[0]
             at = blk.attn
-            b["qkv"] = blk_lin(torch.cat([at.to_q.weight, at.to_k.weight,
-                                          at.to_v.weight]),
-                               torch.cat([at.to_q.bias, at.to_k.bias, at.to_v.bias]))
-            b["cqkv"] = blk_lin(torch.cat([at.add_q_proj.weight, at.add_k_proj.weight,
-                                           at.add_v_proj.weight]),
-                                torch.cat([at.add_q_proj.bias, at.add_k_proj.bias,
-                                           at.add_v_proj.bias]))
+            b["qkv"] = pack_linear(
+                torch.cat([at.to_q.weight, at.to_k.weight, at.to_v.weight]),
+                torch.cat([at.to_q.bias, at.to_k.bias, at.to_v.bias]), dt, dev, fp8)
+            b["cqkv"] = pack_linear(
+                torch.cat([at.add_q_proj.weight, at.add_k_proj.weight, at.add_v_proj.weight]),
+                torch.cat([at.add_q_proj.bias, at.add_k_proj.bias, at.add_v_proj.bias]),
+                dt, dev, fp8)
             b["qk_norm"] = at.qk_norm == "rms_norm"
             if b["qk_norm"]:
-                b["nq"], b["nk"] = f32(at.norm_q.weight), f32(at.norm_k.weight)
-                b["ncq"], b["nck"] = f32(at.norm_added_q.weight), \
-                    f32(at.norm_added_k.weight)
-            b["out"] = blin(at.to_out[0])
+                b["nq"], b["nk"] = fp32(at.norm_q.weight), fp32(at.norm_k.weight)
+                b["ncq"], b["nck"] = fp32(at.norm_added_q.weight), \
+                    fp32(at.norm_added_k.weight)
+            b["out"] = pack_linear(at.to_out[0].weight, at.to_out[0].bias, dt, dev, fp8)
             if not blk.context_pre_only:
-                b["cout"] = blin(at.to_add_out)
-                b["cff1"], b["cff2"] = blin(blk.ff_context.net[0].proj), \
-                    blin(blk.ff_context.net[2])
+                b["cout"], b["cff1"], b["cff2"] = (
+                    pack_linear(m.weight, m.bias, dt, dev, fp8) for m in (
+                        at.to_add_out, blk.ff_context.net[0].proj, blk.ff_context.net[2]))
             if blk.dual:
                 a2 = blk.attn2
-                b["qkv2"] = blk_lin(torch.cat([a2.to_q.weight, a2.to_k.weight,
-                                               a2.to_v.weight]),
-                                    torch.cat([a2.to_q.bias, a2.to_k.bias,
-                                               a2.to_v.bias]))
+                b["qkv2"] = pack_linear(
+                    torch.cat([a2.to_q.weight, a2.to_k.weight, a2.to_v.weight]),
+                    torch.cat([a2.to_q.bias, a2.to_k.bias, a2.to_v.bias]), dt, dev, fp8)
                 if b["qk_norm"]:
-                    b["nq2"], b["nk2"] = f32(a2.norm_q.weight), \
-                        f32(a2.norm_k.weight)
-                b["out2"] = blin(a2.to_out[0])
-            b["ff1"], b["ff2"] = blin(blk.ff.net[0].proj), blin(blk.ff.net[2])
+                    b["nq2"], b["nk2"] = fp32(a2.norm_q.weight), fp32(a2.norm_k.weight)
+                b["out2"] = pack_linear(a2.to_out[0].weight, a2.to_out[0].bias, dt, dev, fp8)
+            b["ff1"], b["ff2"] = (pack_linear(m.weight, m.bias, dt, dev, fp8)
+                                  for m in (blk.ff.net[0].proj, blk.ff.net[2]))
             blocks.append(b)
         mod_w.append(self.norm_out.linear.weight.detach())
         mod_b.append(self.norm_out.linear.bias.detach())
         pk["final_mod"] = (off, 2 * D)
         off += 2 * D
-        pk["mod_w"] = w16(torch.cat(mod_w))
-        pk["mod_b"] = f32(torch.cat(mod_b))
+        pk["mod"] = pack_linear(torch.cat(mod_w), torch.cat(mod_b), dt, dev)
         pk["mod_total"] = off
         pk["blocks"] = blocks
-        pk["proj_out"] = lin(self.proj_out)
+        pk["proj_out"] = pack_linear(self.proj_out.weight, self.proj_out.bias, dt, dev)
         if self.perspective_modeling_type == "implicit":
-            pk["ve1"], pk["ve2"] = lin(self.view_embedding.linear_1), \
-                lin(self.view_embedding.linear_2)
+            pk["ve1"], pk["ve2"] = (pack_linear(m.weight, m.bias, dt, dev) for m in (
+                self.view_embedding.linear_1, self.view_embedding.linear_2))
         if self.enable_crossview:
             pk["cv"] = [b.pack(dt, dev, fp8) for b in self.crossview_transformer_blocks]
-            pk["vpe"] = [(lin(m.linear_1), lin(m.linear_2))
+            pk["vpe"] = [tuple(pack_linear(lin.weight, lin.bias, dt, dev)
+                               for lin in (m.linear_1, m.linear_2))
                          for m in self.view_pos_embeds]
         if self.enable_temporal:
             pk["tp"] = [b.pack(dt, dev, fp8) for b in self.temporal_transformer_blocks]
-            pk["tpe"] = [(lin(m.linear_1), lin(m.linear_2))
+            pk["tpe"] = [tuple(pack_linear(lin.weight, lin.bias, dt, dev)
+                               for lin in (m.linear_1, m.linear_2))
                          for m in self.time_pos_embeds]
         # weight bytes the E4M3 copies save against 16-bit ones (scales included)
-        pk["fp8_bytes_saved"] += sum(p["fp8_bytes_saved"] for p in pk.get("cv", []) + pk.get("tp", []))
+        pk["fp8_bytes_saved"] = fp8_bytes_saved(pk)
         self._pk = pk
         return pk
 
@@ -406,14 +385,18 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
             "tokens": e(N * S, self.patch_size ** 2 * self.out_channels,
                         dtype=torch.float32),
         }
+        # GEMM operands: the LayerNorm outputs (a, ab sample rows, ac context rows) and the
+        # E4M3 buffers the 16-bit GEMM outputs are requantized into (q sample rows, qc
+        # context rows; None in 16 bit)
         if pk["fp8"]:
-            # E4M3 operands + row scales: LayerNorm outputs (a8*, ac8) and the quantized
-            # 16-bit GEMM outputs (q8 sample rows, qc8 context rows)
-            f8 = torch.float8_e4m3fn
-            for k, rows, cols in (("a8", N * S, D), ("a8b", N * S, D), ("ac8", N * L, D),
-                                  ("q8", N * S, 4 * D), ("qc8", N * L, 4 * D)):
-                ws[k] = e(rows, cols, dtype=f8)
-                ws[k + "_s"] = e(rows, dtype=torch.float32)
+            ws["a"], ws["ab"], ws["ac"], ws["q"], ws["qc"] = (
+                Operand(e(rows, cols, dtype=FP8), e(rows, dtype=torch.float32))
+                for rows, cols in ((N * S, D), (N * S, D), (N * L, D), (N * S, 4 * D),
+                                   (N * L, 4 * D)))
+        else:
+            ws["a"], ws["ab"], ws["ac"] = Operand(ws["a16"]), Operand(ws["a16b"]), \
+                Operand(ws["ac16"])
+            ws["q"] = ws["qc"] = None
         self._ws = {key: ws}  # keep a single live workspace
         return ws
 
@@ -424,10 +407,9 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
             (t.data_ptr(), tuple(t.shape), t.dtype, t._version)
 
     def _mlp_run(self, a16, l1, l2, resid=None):
-        h = _ops.linear(a16, l1[0], l1[1], act=_lib.ACT_SILU)
-        return _ops.linear(h, l2[0], l2[1],
-                           epilogue=_lib.EPI_RESID if resid is not None
-                           else _lib.EPI_F32, resid=resid)
+        h = gemm(a16, l1, act=_lib.ACT_SILU)
+        return gemm(h, l2, epilogue=_lib.EPI_RESID if resid is not None else _lib.EPI_F32,
+                    resid=resid)
 
     @torch.no_grad()
     def _conditions(self, B, T, V, Hp, Wp, t_offset, T_total,
@@ -460,9 +442,8 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         ehs = encoder_hidden_states.flatten(0, 2)
         L = ehs.shape[1]
         cd["L"] = L
-        cd["c0"] = _ops.linear(
-            ehs.reshape(N * L, -1).to(dt).contiguous(), pk["ctx"][0], pk["ctx"][1],
-            epilogue=_lib.EPI_F32)
+        cd["c0"] = gemm(ehs.reshape(N * L, -1).to(dt).contiguous(), pk["ctx"],
+                        epilogue=_lib.EPI_F32)
         cd["text_emb"] = self._mlp_run(
             pooled_projections.flatten(0, 2).to(dt).contiguous(),
             pk["p1"], pk["p2"])
@@ -662,13 +643,13 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         remap = dict(rows_per_item=T_loc * V * S, out_item_stride=T * V * S,
                      out_row_offset=plan.t_offset * V * S)
 
-        def project(p, a16, w, nw, out, peer_out=None, **kw):
+        def project(p, a, w, nw, out, peer_out=None, **kw):
             if p["qk_norm"]:
-                gemm(a16, w, epilogue=_lib.EPI_QKNORM, out=out,
+                gemm(a, w, epilogue=_lib.EPI_QKNORM, out=out,
                      q_norm_weight=nw, qk_region=D, qk_norm_regions=1,
                      eps=eps, peer_out=peer_out, **kw)
             else:
-                gemm(a16, w, out=out, peer_out=peer_out, **kw)
+                gemm(a, w, out=out, peer_out=peer_out, **kw)
 
         def attend(kv_all, out):
             if kind == "full":         # (b v) (t hw)
@@ -693,19 +674,20 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
                     kv_group_strides=[T * V * S, 1], seq_kv=T, inner_kv=1,
                     kv_stride_outer=V * S, kv_stride_inner=0)
 
-        def qkv_attend(p, a16, out):
+        def qkv_attend(p, a, out):
+            q, kv = p["qkv"].rows(0, D), p["qkv"].rows(D, 3 * D)
             if peer_kv is not None:
                 # fused: the K,V GEMM epilogue scatters its tiles into every peer's
                 # gathered buffer over NVLink; one group barrier publishes them
                 kv_all, peers, hdl = peer_kv.next()
-                project(p, a16, packed(p, "kv"), p.get("nk"), kv_all, peers, **remap)
-                project(p, a16, packed(p, "q"), p.get("nq"), q_loc)
+                project(p, a, kv, p.get("nk"), kv_all, peers, **remap)
+                project(p, a, q, p.get("nq"), q_loc)
                 hdl.barrier(channel=0)
             else:
                 kv_loc, kv_all = ws["kv_loc"], ws["kv_all"]
-                project(p, a16, packed(p, "kv"), p.get("nk"), kv_loc)
+                project(p, a, kv, p.get("nk"), kv_loc)
                 work = plan.gather_frames_kv(kv_loc, kv_all, batch=B, async_op=True)
-                project(p, a16, packed(p, "q"), p.get("nq"), q_loc)
+                project(p, a, q, p.get("nq"), q_loc)
                 work.wait()
             attend(kv_all, out)
         return qkv_attend
@@ -717,22 +699,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         c_src = ws.pop("c_in", None)          # first block: context read from the cache
         c_src = c if c_src is None else c_src
         qkv, o16, oc16 = ws["qkv_j"], ws["o16"], ws["oc16"]
-        fp8 = self._pk["fp8"]
-        if fp8:   # LayerNorms write E4M3 operands with row scales
-            a16, a16b, ac16 = [(ws[k], ws[k + "_s"]) for k in ("a8", "a8b", "ac8")]
-        else:
-            a16, a16b, ac16 = ws["a16"], ws["a16b"], ws["ac16"]
-
-        def ln(src, dst, **kw):
-            if fp8:
-                if "out2" in kw:
-                    kw["out2"], kw["out2_scale"] = kw["out2"]
-                _ops.layernorm(src, dst[0], out_scale=dst[1], **kw)
-            else:
-                _ops.layernorm(src, dst, **kw)
-
-        def operand(t, key):    # the 16-bit GEMM output t as the next GEMM's operand
-            return fp8_operand(ws, key, t) if fp8 else t
+        a, ab, ac, q, qc = ws["a"], ws["ab"], ws["ac"], ws["q"], ws["qc"]
         o, _ = b["mod"]
         m = [mod[:, o + i * D:o + (i + 1) * D] for i in range(9 if b["dual"] else 6)]
         shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp = m[:6]
@@ -745,53 +712,53 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
                 c_gate_mlp = cm
         kw = {}
         if b["dual"]:
-            kw = dict(shift2=m[6], scale2=m[7], out2=a16b)
+            kw = dict(shift2=m[6], scale2=m[7], out2=ab)
         if residual is not None:   # hidden_states += condition residual (:491-494)
             kw.update(add_full=residual, sum_out=x)
-        ln(x, a16, eps=1e-6, rows_per_item=S, shift=shift_msa, scale=scale_msa, **kw)
-        ln(c_src, ac16, eps=1e-6, rows_per_item=L, shift=c_shift_msa, scale=c_scale_msa)
+        layernorm(x, a, eps=1e-6, rows_per_item=S, shift=shift_msa, scale=scale_msa, **kw)
+        layernorm(c_src, ac, eps=1e-6, rows_per_item=L, shift=c_shift_msa, scale=c_scale_msa)
         if b["qk_norm"]:
-            gemm(a16, b["qkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
+            gemm(a, b["qkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
                  rows_per_item=S, out_item_stride=S + L, out_row_offset=0,
                  q_norm_weight=b["nq"], k_norm_weight=b["nk"], qk_region=D,
                  eps=1e-6)
-            gemm(ac16, b["cqkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
+            gemm(ac, b["cqkv"], epilogue=_lib.EPI_QKNORM, out=qkv,
                  rows_per_item=L, out_item_stride=S + L, out_row_offset=S,
                  q_norm_weight=b["ncq"], k_norm_weight=b["nck"],
                  qk_region=D, eps=1e-6)
         else:
-            gemm(a16, b["qkv"], out=qkv, rows_per_item=S,
+            gemm(a, b["qkv"], out=qkv, rows_per_item=S,
                  out_item_stride=S + L, out_row_offset=0)
-            gemm(ac16, b["cqkv"], out=qkv, rows_per_item=L,
+            gemm(ac, b["cqkv"], out=qkv, rows_per_item=L,
                  out_item_stride=S + L, out_row_offset=S)
         # joint attention over [sample ; context] tokens of each view-frame
         _ops.attention(qkv, o16, D=D, heads=heads, group_dims=[N],
                        group_strides=[S + L], seq=S + L, out_group_strides=[S],
                        out_stride_outer=0, out_stride_inner=1, split=S, out2=oc16)
-        gemm(operand(o16, "q8"), b["out"], epilogue=_lib.EPI_RESID, resid=x, out=x,
+        gemm(requantize(o16, q), b["out"], epilogue=_lib.EPI_RESID, resid=x, out=x,
              gate=gate_msa, rows_per_item=S)
         if b["dual"]:
             q2 = ws["qkv_s"]
             if b["qk_norm"]:
-                gemm(a16b, b["qkv2"], epilogue=_lib.EPI_QKNORM, out=q2,
+                gemm(ab, b["qkv2"], epilogue=_lib.EPI_QKNORM, out=q2,
                      q_norm_weight=b["nq2"], k_norm_weight=b["nk2"],
                      qk_region=D, eps=1e-6)
             else:
-                gemm(a16b, b["qkv2"], out=q2)
+                gemm(ab, b["qkv2"], out=q2)
             _ops.attention(q2, o16, D=D, heads=heads, group_dims=[N],
                            group_strides=[S], seq=S)
-            gemm(operand(o16, "q8"), b["out2"], epilogue=_lib.EPI_RESID, resid=x, out=x,
+            gemm(requantize(o16, q), b["out2"], epilogue=_lib.EPI_RESID, resid=x, out=x,
                  gate=m[8], rows_per_item=S)
-        ln(x, a16, eps=1e-6, rows_per_item=S, shift=shift_mlp, scale=scale_mlp)
-        gemm(a16, b["ff1"], act=_lib.ACT_GELU_TANH, out=ws["g16"])
-        gemm(operand(ws["g16"], "q8"), b["ff2"], epilogue=_lib.EPI_RESID, resid=x, out=x,
+        layernorm(x, a, eps=1e-6, rows_per_item=S, shift=shift_mlp, scale=scale_mlp)
+        gemm(a, b["ff1"], act=_lib.ACT_GELU_TANH, out=ws["g16"])
+        gemm(requantize(ws["g16"], q), b["ff2"], epilogue=_lib.EPI_RESID, resid=x, out=x,
              gate=gate_mlp, rows_per_item=S)
         if not b["last"]:
-            gemm(operand(oc16, "qc8"), b["cout"], epilogue=_lib.EPI_RESID, resid=c_src,
+            gemm(requantize(oc16, qc), b["cout"], epilogue=_lib.EPI_RESID, resid=c_src,
                  out=c, gate=c_gate_msa, rows_per_item=L)
-            ln(c, ac16, eps=1e-6, rows_per_item=L, shift=c_shift_mlp, scale=c_scale_mlp)
-            gemm(ac16, b["cff1"], act=_lib.ACT_GELU_TANH, out=ws["gc16"])
-            gemm(operand(ws["gc16"], "qc8"), b["cff2"], epilogue=_lib.EPI_RESID, resid=c,
+            layernorm(c, ac, eps=1e-6, rows_per_item=L, shift=c_shift_mlp, scale=c_scale_mlp)
+            gemm(ac, b["cff1"], act=_lib.ACT_GELU_TANH, out=ws["gc16"])
+            gemm(requantize(ws["gc16"], qc), b["cff2"], epilogue=_lib.EPI_RESID, resid=c,
                  out=c, gate=c_gate_mlp, rows_per_item=L)
 
     # -- forward -------------------------------------------------------------------------------
@@ -834,9 +801,8 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         n1 = (N // cfg_repeat) * S
         for r in range(cfg_repeat):
             _ops.patchify(x_in, P, ws["patch16"][r * n1:(r + 1) * n1])
-        _ops.linear(ws["patch16"], pk["patch_w"], pk["patch_b"],
-                    epilogue=_lib.EPI_RESID, resid=cd["pos"], resid_row_mod=S,
-                    out=ws["x"])
+        gemm(ws["patch16"], pk["patch"], epilogue=_lib.EPI_RESID, resid=cd["pos"],
+             resid_row_mod=S, out=ws["x"])
         # K3: temb = timestep_embedder(sinusoid(t)) + text_embedder(pooled)
         t_in = timestep.flatten()
         if t_in.dtype != torch.float32 or not t_in.is_contiguous():
@@ -844,13 +810,11 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         for r in range(cfg_repeat):
             _ops.sinusoid(t_in, 256, ws["tsin"][r * t_in.numel():(r + 1) * t_in.numel()],
                           True, 0.0)
-        _ops.linear(ws["tsin"], *pk["t1"], act=_lib.ACT_SILU, out=ws["th"])
-        _ops.linear(ws["th"], *pk["t2"], epilogue=_lib.EPI_RESID,
-                    resid=cd["text_emb"], out=ws["temb"])
+        gemm(ws["tsin"], pk["t1"], act=_lib.ACT_SILU, out=ws["th"])
+        gemm(ws["th"], pk["t2"], epilogue=_lib.EPI_RESID, resid=cd["text_emb"], out=ws["temb"])
         _ops.act_cast(ws["temb"], ws["temb_silu"], _lib.ACT_SILU)
         # every AdaLN modulation of the forward in one GEMM
-        _ops.linear(ws["temb_silu"], pk["mod_w"], pk["mod_b"],
-                    epilogue=_lib.EPI_F32, out=ws["mod"])
+        gemm(ws["temb_silu"], pk["mod"], epilogue=_lib.EPI_F32, out=ws["mod"])
         # the context stream starts as the (cached, read-only) embedded text: block 0 reads
         # cd["c0"] and writes ws["c"], so no per-step copy of it is made
         ws["c_in"] = cd["c0"]
@@ -890,8 +854,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         _ops.layernorm(ws["x"], ws["a16"], eps=1e-6, rows_per_item=S,
                        scale=ws["mod"][:, fo:fo + D],
                        shift=ws["mod"][:, fo + D:fo + 2 * D])
-        _ops.linear(ws["a16"], *pk["proj_out"], epilogue=_lib.EPI_F32,
-                    out=ws["tokens"])
+        gemm(ws["a16"], pk["proj_out"], epilogue=_lib.EPI_F32, out=ws["tokens"])
         return ws["tokens"], (B, T, V, Hp, Wp)
 
     def forward(

@@ -22,8 +22,9 @@ from opendwm_b200 import ops as _ops
 from .. import _compat
 from . import adapters as _adapters
 from .crossview_temporal import (
-    AlphaBlender, ParamGroup, VTSelfAttentionBlock, fp8_operand, gemm, make_attention,
-    make_feed_forward)
+    AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward)
+from .packing import (
+    FP8, Operand, conv, gemm, layernorm, pack_conv, pack_linear, pack_norm, requantize)
 
 
 def _mlp(i, h, o):
@@ -288,40 +289,6 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         dt = self._dtype()
         fp8 = self.gemm_dtype is not None
 
-        def f32(t):
-            return t.detach().to(dev, torch.float32).contiguous()
-
-        def lin(m):
-            return (m.weight.detach().to(dev, dt).contiguous(),
-                    None if m.bias is None else f32(m.bias))
-
-        def lin8(w, b):
-            """`gemm` weight tuple of a block linear: E4M3 + channel scales with gemm_dtype,
-            else 16-bit (b: fp32 or None)."""
-            if not fp8:
-                return w.detach().to(dev, dt).contiguous(), b
-            w8, s = _ops.quantize_weight_rows(w.to(dev))
-            return w8, b, s, dt
-
-        def conv8(m):
-            """A ResBlock conv: E4M3 tap-major weight + bias + channel scales with gemm_dtype."""
-            if not fp8:
-                return conv(m)
-            w8, s = _ops.pack_conv_weight_fp8(m.weight.to(dev))
-            return w8, f32(m.bias), s
-
-        def conv(m, pad_out=None, pad_in=None):
-            w = _ops.pack_conv_weight(m.weight.to(dev), dt, pad_out_to=pad_out, pad_in_to=pad_in)
-            b = f32(m.bias)
-            if pad_out and pad_out != b.numel():
-                bp = torch.zeros(pad_out, device=dev)
-                bp[:b.numel()] = b
-                b = bp
-            return w, b
-
-        def gn(m):
-            return f32(m.weight), f32(m.bias), m.eps
-
         temb_w, temb_b, off = [], [], [0]
 
         def temb_slot(linear):
@@ -333,46 +300,48 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
 
         def res(rb):
             s = rb.spatial_res_block
-            p = dict(n1=gn(s.norm1), c1=conv8(s.conv1), temb=temb_slot(s.time_emb_proj),
-                     n2=gn(s.norm2), c2=conv8(s.conv2))
+            p = dict(n1=pack_norm(s.norm1), c1=pack_conv(s.conv1, dt, dev, fp8),
+                     temb=temb_slot(s.time_emb_proj), n2=pack_norm(s.norm2),
+                     c2=pack_conv(s.conv2, dt, dev, fp8))
             if hasattr(s, "conv_shortcut"):
-                c = s.conv_shortcut
-                p["sc"] = (c.weight.detach().reshape(c.out_channels, -1).to(dev, dt).contiguous(),
-                           f32(c.bias))
+                p["sc"] = pack_linear(s.conv_shortcut.weight, s.conv_shortcut.bias, dt, dev)
             if rb.temporal_res_block is not None:
                 t = rb.temporal_res_block
-                p["t"] = dict(n1=gn(t.norm1), c1=conv8(t.conv1), temb=temb_slot(t.time_emb_proj),
-                              n2=gn(t.norm2), c2=conv8(t.conv2))
+                p["t"] = dict(n1=pack_norm(t.norm1), c1=pack_conv(t.conv1, dt, dev, fp8),
+                              temb=temb_slot(t.time_emb_proj), n2=pack_norm(t.norm2),
+                              c2=pack_conv(t.conv2, dt, dev, fp8))
             return p
 
         def attn(tm):
-            p = dict(norm=gn(tm.norm), proj_in=lin(tm.proj_in), proj_out=lin(tm.proj_out),
+            p = dict(norm=pack_norm(tm.norm),
+                     proj_in=pack_linear(tm.proj_in.weight, tm.proj_in.bias, dt, dev),
+                     proj_out=pack_linear(tm.proj_out.weight, tm.proj_out.bias, dt, dev),
                      blocks=[])
             for b in tm.transformer_blocks:
                 a1, a2 = b.attn1, b.attn2
-
-                def blin(m):
-                    return lin8(m.weight.detach(), None if m.bias is None else f32(m.bias))
                 ff1_w, ff1_b = _ops.pack_geglu(b.ff.net[0].proj.weight.detach().to(dev),
                                                b.ff.net[0].proj.bias.detach().to(dev))
                 p["blocks"].append(dict(
-                    n1=(f32(b.norm1.weight), f32(b.norm1.bias), b.norm1.eps),
-                    qkv=lin8(torch.cat([a1.to_q.weight, a1.to_k.weight, a1.to_v.weight])
-                             .detach(), None),
-                    out=blin(a1.to_out[0]),
-                    n2=(f32(b.norm2.weight), f32(b.norm2.bias), b.norm2.eps),
-                    q2=blin(a2.to_q),
-                    kv2=torch.cat([a2.to_k.weight, a2.to_v.weight]).detach().to(dev, dt).contiguous(),
-                    out2=blin(a2.to_out[0]),
-                    n3=(f32(b.norm3.weight), f32(b.norm3.bias), b.norm3.eps),
+                    n1=pack_norm(b.norm1),
+                    qkv=pack_linear(torch.cat([a1.to_q.weight, a1.to_k.weight, a1.to_v.weight]),
+                                    None, dt, dev, fp8),
+                    out=pack_linear(a1.to_out[0].weight, a1.to_out[0].bias, dt, dev, fp8),
+                    n2=pack_norm(b.norm2),
+                    q2=pack_linear(a2.to_q.weight, a2.to_q.bias, dt, dev, fp8),
+                    # the step-invariant text K,V projection stays 16-bit
+                    kv2=pack_linear(torch.cat([a2.to_k.weight, a2.to_v.weight]), None, dt, dev),
+                    out2=pack_linear(a2.to_out[0].weight, a2.to_out[0].bias, dt, dev, fp8),
+                    n3=pack_norm(b.norm3),
                     # FP8: quantized after the GEGLU row packing, scales follow the rows
-                    ff1=lin8(ff1_w, ff1_b.float().contiguous()),
-                    ff2=blin(b.ff.net[2])))
+                    ff1=pack_linear(ff1_w, ff1_b, dt, dev, fp8),
+                    ff2=pack_linear(b.ff.net[2].weight, b.ff.net[2].bias, dt, dev, fp8)))
             if tm.view_pos_embed is not None:
-                p["vpe"] = (lin(tm.view_pos_embed.linear_1), lin(tm.view_pos_embed.linear_2))
+                p["vpe"] = tuple(pack_linear(m.weight, m.bias, dt, dev) for m in (
+                    tm.view_pos_embed.linear_1, tm.view_pos_embed.linear_2))
                 p["cv"] = [b.pack(dt, dev, fp8) for b in tm.crossview_transformer_blocks]
             if tm.time_pos_embed is not None:
-                p["tpe"] = (lin(tm.time_pos_embed.linear_1), lin(tm.time_pos_embed.linear_2))
+                p["tpe"] = tuple(pack_linear(m.weight, m.bias, dt, dev) for m in (
+                    tm.time_pos_embed.linear_1, tm.time_pos_embed.linear_2))
                 p["tp"] = [b.pack(dt, dev, fp8) for b in tm.temporal_transformer_blocks]
             return p
 
@@ -380,23 +349,25 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             p = dict(res=[res(r) for r in b.resnets],
                      attn=None if b.attentions is None else [attn(a) for a in b.attentions])
             if hasattr(b, "downsamplers"):
-                p["down"] = conv(b.downsamplers[0].conv)
+                p["down"] = pack_conv(b.downsamplers[0].conv, dt, dev)
             if hasattr(b, "upsamplers"):
-                p["up"] = conv(b.upsamplers[0].conv)
+                p["up"] = pack_conv(b.upsamplers[0].conv, dt, dev)
             return p
 
         cin_p = (self.in_channels + 7) // 8 * 8
         pk = dict(dtype=dt, fp8=fp8, cin_p=cin_p,
-                  conv_in=conv(self.conv_in, pad_in=cin_p),
-                  te=(lin(self.time_embedding.linear_1), lin(self.time_embedding.linear_2)),
+                  conv_in=pack_conv(self.conv_in, dt, dev, pad_in=cin_p),
+                  te=tuple(pack_linear(m.weight, m.bias, dt, dev) for m in (
+                      self.time_embedding.linear_1, self.time_embedding.linear_2)),
                   down=[block(b) for b in self.down_blocks], mid=block(self.mid_block),
                   up=[block(b) for b in self.up_blocks],
-                  norm_out=gn(self.conv_norm_out),
-                  conv_out=conv(self.conv_out, pad_out=32 if self.out_channels < 32 else None))
+                  norm_out=pack_norm(self.conv_norm_out),
+                  conv_out=pack_conv(self.conv_out, dt, dev,
+                                     pad_out=32 if self.out_channels < 32 else None))
         if self.add_embedding is not None:
-            pk["ae"] = (lin(self.add_embedding.linear_1), lin(self.add_embedding.linear_2))
-        pk["temb_w"] = torch.cat(temb_w).to(dev, dt).contiguous()
-        pk["temb_b"] = torch.cat(temb_b).float().to(dev).contiguous()
+            pk["ae"] = tuple(pack_linear(m.weight, m.bias, dt, dev) for m in (
+                self.add_embedding.linear_1, self.add_embedding.linear_2))
+        pk["temb"] = pack_linear(torch.cat(temb_w), torch.cat(temb_b), dt, dev)
         self._pk = pk
         return pk
 
@@ -419,44 +390,41 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             self._ws8[k] = torch.zeros(shape, device=self.conv_in.weight.device, dtype=dtype)
         return self._ws8[k]
 
-    def _gn8(self, x5, g, out_T=None, out_t0=0):
-        """GroupNorm(32)+SiLU of fp32 [nb, T, H, W, C] as an FP8 conv operand: (E4M3
-        [nb, out_T, H, W, C], fp32 scales [nb]), one scale per volume nb.  Frames outside
-        [out_t0, out_t0 + T) stay zero."""
+    def _norm_act(self, x5, g, out_T=None, out_t0=0):
+        """GroupNorm(32)+SiLU of fp32 [nb, T, H, W, C] as a conv operand [nb, out_T, H, W, C]
+        whose frames outside [out_t0, out_t0 + T) are zero: 16-bit, or with gemm_dtype E4M3
+        with one fp32 scale per volume nb (in the persistent `_buf8` workspace)."""
         nb, T, H, W, C = x5.shape
         out_T = T if out_T is None else out_T
         sums = _ops.groupnorm_stats(x5, 32)
-        out = self._buf8("gn", (nb, out_T, H, W, C), torch.float8_e4m3fn)
-        sc = self._buf8("gn_s", (nb,), torch.float32)
-        return _ops.groupnorm_silu_e4m3(x5, sums, g[0], g[1], out, sc, groups=32, eps=g[2],
-                                        out_t0=out_t0, silu=True)
-
-    @staticmethod
-    def _conv(a, c, **kw):
-        """ResBlock conv of operand `a` (16-bit, or _gn8's (E4M3, scales)) with packed c."""
-        if len(c) == 3:
-            return _ops.conv(a[0], c[0], c[1], a_scale=a[1], w_scale=c[2], **kw)
-        return _ops.conv(a, *c, **kw)
+        if self._pk["fp8"]:
+            out = self._buf8("gn", (nb, out_T, H, W, C), FP8)
+            sc = self._buf8("gn_s", (nb,), torch.float32)
+            return Operand(*_ops.groupnorm_silu_e4m3(x5, sums, g[0], g[1], out, sc, groups=32,
+                                                     eps=g[2], out_t0=out_t0, silu=True))
+        # a fresh buffer per call; the frames a temporal conv pads with must be zero
+        out = (torch.empty if out_T == T else torch.zeros)(
+            nb, out_T, H, W, C, device=x5.device, dtype=self._pk["dtype"])
+        return _ops.spatialnorm_silu(x5, sums, g[0], g[1], out, groups=32, eps=g[2],
+                                     out_t0=out_t0, silu=True)
 
     def _resblock(self, p, h, N, H, W, temb_all, geo, dis_t, alpha_mod):
         S = H * W
 
-        def norm_act(t, g):    # conv operand: 16-bit, or E4M3 with one scale per item
-            if self._pk["fp8"]:
-                return self._gn8(t.view(N, 1, H, W, t.shape[1]), g)
-            return self._gn(t, N, H, W, g, True)
+        def norm_act(t, g):    # one scale per item in E4M3
+            return self._norm_act(t.view(N, 1, H, W, t.shape[1]), g)
         a = norm_act(h, p["n1"])
         o, n = p["temb"]
-        h1 = self._conv(a, p["c1"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID,
-                        resid=temb_all[:, o:o + n], resid_rows_per_item=S)
+        h1 = conv(a, p["c1"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID,
+                  resid=temb_all[:, o:o + n], resid_rows_per_item=S)
         b = norm_act(h1, p["n2"])
         if "sc" in p:
             h16 = torch.empty(h.shape, device=h.device, dtype=self._pk["dtype"])
             _ops.act_cast(h, h16)
-            skip = _ops.linear(h16, *p["sc"], epilogue=_lib.EPI_F32)
+            skip = gemm(h16, p["sc"], epilogue=_lib.EPI_F32)
         else:
             skip = h
-        out = self._conv(b, p["c2"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID, resid=skip)
+        out = conv(b, p["c2"], kernel=(1, 3, 3), epilogue=_lib.EPI_RESID, resid=skip)
         if "t" in p and not dis_t["all"]:
             out = self._temporal_res(p["t"], out, N, H, W, temb_all, geo, alpha_mod)
         return out
@@ -465,28 +433,22 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         """TemporalResnetBlock (conv3d (3,1,1), GroupNorm over (T,H,W)) + AlphaBlender on
         the `(b v) t` volumes; (b t v) <-> (b v t) regrouping is a data-movement permute."""
         B, T, V = geo
-        S, C, dt = H * W, x.shape[1], self._pk["dtype"]
+        S, C = H * W, x.shape[1]
         xp = x.view(B, T, V, S, C).permute(0, 2, 1, 3, 4).contiguous()      # [B,V,T,S,C]
         x5 = xp.view(B * V, T, 1, S, C)
         o, n = p["temb"]
         temb_p = temb_all[:, o:o + n].reshape(B, T, V, n).permute(0, 2, 1, 3)\
             .reshape(B * V * T, n).contiguous()
 
-        def norm_act(t5, g):
-            if self._pk["fp8"]:     # E4M3 with one scale per (b v) volume of T frames
-                return self._gn8(t5, g, out_T=T + 2, out_t0=1)
-            sums = _ops.groupnorm_stats(t5, 32)
-            buf = torch.zeros(B * V, T + 2, 1, S, C, device=x.device, dtype=dt)
-            _ops.spatialnorm_silu(t5, sums, g[0], g[1], buf, groups=32, eps=g[2], out_t0=1,
-                                  silu=True)
-            return buf
-        h1 = self._conv(norm_act(x5, p["n1"]), p["c1"], kernel=(3, 1, 1),
-                        epilogue=_lib.EPI_RESID, resid=temb_p, resid_rows_per_item=S)
+        def norm_act(t5, g):    # T + 2 frames, zero at both ends; E4M3: one scale per (b v)
+            return self._norm_act(t5, g, out_T=T + 2, out_t0=1)
+        h1 = conv(norm_act(x5, p["n1"]), p["c1"], kernel=(3, 1, 1),
+                  epilogue=_lib.EPI_RESID, resid=temb_p, resid_rows_per_item=S)
         xr = xp.view(B * V * T * S, C)
         alpha = mixer["alpha"]
-        y = self._conv(norm_act(h1.view(B * V, T, 1, S, C), p["n2"]), p["c2"],
-                       kernel=(3, 1, 1), epilogue=_lib.EPI_RESID, resid=xr, blend_x=xr,
-                       alpha=alpha, rows_per_batch=V * T * S)
+        y = conv(norm_act(h1.view(B * V, T, 1, S, C), p["n2"]), p["c2"],
+                 kernel=(3, 1, 1), epilogue=_lib.EPI_RESID, resid=xr, blend_x=xr,
+                 alpha=alpha, rows_per_batch=V * T * S)
         return y.view(B, V, T, S, C).permute(0, 2, 1, 3, 4).reshape(B * T * V * S, C)\
             .contiguous()
 
@@ -494,8 +456,8 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         idx = torch.arange(count, device=dev, dtype=torch.float32)
         sn = torch.empty(count, C, device=dev, dtype=dt)
         _ops.sinusoid(idx, C, sn, True, 0.0)
-        hmid = _ops.linear(sn, *mlp[0], act=_lib.ACT_SILU)
-        return _ops.linear(hmid, *mlp[1], epilogue=_lib.EPI_F32)
+        hmid = gemm(sn, mlp[0], act=_lib.ACT_SILU)
+        return gemm(hmid, mlp[1], epilogue=_lib.EPI_F32)
 
     def _transformer(self, tm, p, x, N, H, W, geo, cd, level_key):
         """TransformerModel forward on fp32 tokens x [N*S, C]; returns x + proj_out(...)."""
@@ -503,31 +465,22 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         S, dt, dev = H * W, self._pk["dtype"], x.device
         inner, heads = tm.inner_dim, tm.heads
         a16 = self._gn(x, N, H, W, p["norm"], False).view(N * S, -1)
-        h = _ops.linear(a16, *p["proj_in"], epilogue=_lib.EPI_F32)
+        h = gemm(a16, p["proj_in"], epilogue=_lib.EPI_F32)
         ws = dict(y=torch.empty_like(h), a16=torch.empty(N * S, inner, device=dev, dtype=dt),
                   g16=torch.empty(N * S, 4 * inner, device=dev, dtype=dt),
                   qkv_s=torch.empty(N * S, 3 * inner, device=dev, dtype=dt),
                   o16=torch.empty(N * S, inner, device=dev, dtype=dt))
-        fp8 = self._pk["fp8"]
-        if fp8:
-            # E4M3 operands + row scales: LayerNorm outputs (a8) and the quantized 16-bit
-            # attention / GEGLU outputs (q8); the VTSelfAttentionBlocks use the same keys
-            f8 = torch.float8_e4m3fn
-            for k, cols in (("a8", inner), ("q8", 4 * inner)):
-                ws[k] = self._buf8(k, (N * S, cols), f8)
-                ws[k + "_s"] = self._buf8(k + "_s", (N * S,), torch.float32)
-            a = (ws["a8"], ws["a8_s"])
+        # GEMM operands: the LayerNorm output (a) and the E4M3 buffer the 16-bit attention /
+        # GEGLU outputs are requantized into (q; None in 16 bit); the VTSelfAttentionBlocks
+        # use the same keys
+        if self._pk["fp8"]:
+            ws["a"], ws["q"] = (
+                Operand(self._buf8(k, (N * S, cols), FP8),
+                        self._buf8(k + "_s", (N * S,), torch.float32))
+                for k, cols in (("a8", inner), ("q8", 4 * inner)))
         else:
-            a = ws["a16"]
-
-        def ln(src, g):
-            if fp8:
-                _ops.layernorm(src, a[0], out_scale=a[1], weight=g[0], bias=g[1], eps=g[2])
-            else:
-                _ops.layernorm(src, a, weight=g[0], bias=g[1], eps=g[2])
-
-        def operand(t):    # the 16-bit GEMM output t as the next GEMM's operand
-            return fp8_operand(ws, "q8", t) if fp8 else t
+            ws["a"], ws["q"] = Operand(ws["a16"]), None
+        a, q = ws["a"], ws["q"]
         ctx = cd["ctx16"]
         Lc = cd["ctx_len"]
         key = (level_key, "tabs")
@@ -545,24 +498,27 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         tabs = cd[key]
         for li, bp in enumerate(p["blocks"]):
             # --- spatial BasicTransformerBlock: self-attn, cross-attn to text, GEGLU FF
-            ln(h, bp["n1"])
+            n = bp["n1"]
+            layernorm(h, a, weight=n[0], bias=n[1], eps=n[2])
             gemm(a, bp["qkv"], out=ws["qkv_s"])
             _ops.attention(ws["qkv_s"], ws["o16"], D=inner, heads=heads, group_dims=[N],
                            group_strides=[S], seq=S)
-            gemm(operand(ws["o16"]), bp["out"], epilogue=_lib.EPI_RESID, resid=h, out=h)
-            ln(h, bp["n2"])
-            q = gemm(a, bp["q2"], out=ws["qkv_s"][:, :inner])
+            gemm(requantize(ws["o16"], q), bp["out"], epilogue=_lib.EPI_RESID, resid=h, out=h)
+            n = bp["n2"]
+            layernorm(h, a, weight=n[0], bias=n[1], eps=n[2])
+            q2 = gemm(a, bp["q2"], out=ws["qkv_s"][:, :inner])
             kkey = (level_key, li, "kv")
             if kkey not in cd:        # text K,V are step-invariant
-                cd[kkey] = _ops.linear(ctx, bp["kv2"], None)
+                cd[kkey] = gemm(ctx, bp["kv2"])
             kv = cd[kkey]
-            _ops.attention(q, ws["o16"], D=inner, heads=heads, group_dims=[N],
+            _ops.attention(q2, ws["o16"], D=inner, heads=heads, group_dims=[N],
                            group_strides=[S], seq=S, kv=kv, k_col=0, v_col=inner,
                            kv_group_strides=[Lc], seq_kv=Lc)
-            gemm(operand(ws["o16"]), bp["out2"], epilogue=_lib.EPI_RESID, resid=h, out=h)
-            ln(h, bp["n3"])
+            gemm(requantize(ws["o16"], q), bp["out2"], epilogue=_lib.EPI_RESID, resid=h, out=h)
+            n = bp["n3"]
+            layernorm(h, a, weight=n[0], bias=n[1], eps=n[2])
             gemm(a, bp["ff1"], epilogue=_lib.EPI_GEGLU, out=ws["g16"])
-            gemm(operand(ws["g16"]), bp["ff2"], epilogue=_lib.EPI_RESID, resid=h, out=h)
+            gemm(requantize(ws["g16"], q), bp["ff2"], epilogue=_lib.EPI_RESID, resid=h, out=h)
             # --- cross-view block
             if "cv" in p and not cd["dis_cv"]["all"]:
                 if tm.enable_rowwise_crossview:   # (bt h) x (v w), view mask per (vq, vk)
@@ -600,7 +556,7 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                     tm.time_mixer.batch_alpha(B, cd["dis_t"]["t"], dev), T * V * S)
         h16 = torch.empty(h.shape, device=dev, dtype=dt)
         _ops.act_cast(h, h16)
-        return _ops.linear(h16, *p["proj_out"], epilogue=_lib.EPI_RESID, resid=x)
+        return gemm(h16, p["proj_out"], epilogue=_lib.EPI_RESID, resid=x)
 
     def _run_block(self, blk, p, h, N, H, W, temb_all, geo, cd, name, skips=None):
         outs = []
@@ -631,8 +587,8 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             C = h.shape[1]
             h16 = torch.empty(h.shape, device=h.device, dtype=dt)
             _ops.act_cast(h, h16)
-            full = _ops.conv(h16.view(N, 1, H, W, C), *p["down"], kernel=(1, 3, 3),
-                             epilogue=_lib.EPI_F32)
+            full = conv(h16.view(N, 1, H, W, C), p["down"], kernel=(1, 3, 3),
+                        epilogue=_lib.EPI_F32)
             h = full.view(N, H, W, C)[:, ::2, ::2].reshape(-1, C).contiguous()
             H, W = (H + 1) // 2, (W + 1) // 2
             outs.append(h)
@@ -640,7 +596,7 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             C = h.shape[1]
             u = _ops.upsample_nearest(h.view(N, 1, H, W, C), False, dt)
             H, W = 2 * H, 2 * W
-            h = _ops.conv(u, *p["up"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+            h = conv(u, p["up"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         return h, outs, H, W
 
     # -- conditions cache ------------------------------------------------------------------------
@@ -671,8 +627,8 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             ids = added_time_ids.flatten().float().contiguous()
             sn = torch.empty(ids.numel(), self.addition_time_embed_dim, device=dev, dtype=dt)
             _ops.sinusoid(ids, self.addition_time_embed_dim, sn, True, 0.0)
-            hm = _ops.linear(sn.view(N, -1), *pk["ae"][0], act=_lib.ACT_SILU)
-            cd["aug"] = _ops.linear(hm, *pk["ae"][1], epilogue=_lib.EPI_F32)
+            hm = gemm(sn.view(N, -1), pk["ae"][0], act=_lib.ACT_SILU)
+            cd["aug"] = gemm(hm, pk["ae"][1], epilogue=_lib.EPI_F32)
 
         def flags(t):
             t = torch.zeros(B, dtype=torch.bool, device=dev) if t is None else \
@@ -720,21 +676,21 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                               added_time_ids, disable_crossview, disable_temporal,
                               crossview_attention_mask)
         # 1. time embeddings: emb = time_embedding(sin(t)) [+ add_embedding(sin(ids))]
-        tsin = torch.empty(N, pk["te"][0][0].shape[1], device=dev, dtype=dt)
+        tsin = torch.empty(N, pk["te"][0].w.shape[1], device=dev, dtype=dt)
         _ops.sinusoid(timesteps.flatten().float().contiguous(), tsin.shape[1], tsin, True, 0.0)
-        hm = _ops.linear(tsin, *pk["te"][0], act=_lib.ACT_SILU)
+        hm = gemm(tsin, pk["te"][0], act=_lib.ACT_SILU)
         if cd["aug"] is not None:
-            emb = _ops.linear(hm, *pk["te"][1], epilogue=_lib.EPI_RESID, resid=cd["aug"])
+            emb = gemm(hm, pk["te"][1], epilogue=_lib.EPI_RESID, resid=cd["aug"])
         else:
-            emb = _ops.linear(hm, *pk["te"][1], epilogue=_lib.EPI_F32)
+            emb = gemm(hm, pk["te"][1], epilogue=_lib.EPI_F32)
         emb16 = torch.empty(emb.shape, device=dev, dtype=dt)
         _ops.act_cast(emb, emb16, _lib.ACT_SILU)
         # every ResBlock's time_emb_proj(SiLU(emb)) in one GEMM
-        temb_all = _ops.linear(emb16, pk["temb_w"], pk["temb_b"], epilogue=_lib.EPI_F32)
+        temb_all = gemm(emb16, pk["temb"], epilogue=_lib.EPI_F32)
         # 2. conv_in on channels-last 16-bit input
         x = torch.zeros(N, 1, H, W, pk["cin_p"], device=dev, dtype=dt)
         x[..., :Cin] = sample.reshape(N, Cin, H, W).permute(0, 2, 3, 1).unsqueeze(1)
-        h = _ops.conv(x, *pk["conv_in"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+        h = conv(x, pk["conv_in"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         residuals = list(cd["residuals"])
         if residuals:
             _ops.axpy(residuals.pop(0), h)
@@ -756,7 +712,7 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             h, _, cH, cW = self._run_block(blk, bp, h, N, cH, cW, temb_all, geo, cd,
                                            ("up", i), skips=res)
         a = self._gn(h, N, cH, cW, pk["norm_out"], True)
-        y = _ops.conv(a, *pk["conv_out"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
+        y = conv(a, pk["conv_out"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
         out = y.view(N, cH, cW, -1)[..., :self.out_channels].permute(0, 3, 1, 2)\
             .reshape(B, T, V, self.out_channels, cH, cW).contiguous()
         out = out.to(sample.dtype if sample.dtype.is_floating_point else torch.float32)

@@ -317,7 +317,7 @@ def test_model_accuracy_against_fake_quant_oracle(which):
     at = o.transformer_blocks[0].attn
     w = torch.cat([at.to_q.weight, at.to_k.weight, at.to_v.weight]).detach()
     q_ref, s_ref = fe.quantize_rows(w)
-    q, s = m._pk["blocks"][0]["qkv"][0], m._pk["blocks"][0]["qkv"][2]
+    q, s = m._pk["blocks"][0]["qkv"].w, m._pk["blocks"][0]["qkv"].scale
     assert torch.equal(q.cpu().view(torch.uint8), q_ref.view(torch.uint8))
     assert torch.equal(s.cpu(), s_ref)
     assert m._pk["fp8_bytes_saved"] > 0

@@ -281,7 +281,7 @@ def test_model_accuracy_against_fake_quant_oracle(case):
     # the packed conv weights are the emulator's: same quantizer on the same fp32 parameters
     conv = o.down_blocks[0].resnets[0].spatial_res_block.conv1
     q_ref, s_ref = fe.quantize_rows(conv.weight.detach().float().reshape(conv.out_channels, -1).cpu())
-    w8, _, s = m._pk["down"][0]["res"][0]["c1"]
+    w8, s = m._pk["down"][0]["res"][0]["c1"].w, m._pk["down"][0]["res"][0]["c1"].scale
     assert torch.equal(s.cpu(), s_ref)
     assert torch.equal(w8.permute(1, 0, 2).reshape(conv.out_channels, -1).cpu().view(torch.uint8),
                        q_ref.view(conv.out_channels, conv.in_channels, 9).transpose(1, 2)
