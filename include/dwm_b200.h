@@ -18,6 +18,11 @@
  *    opt-in 8-bit GEMM operands are E4M3 (DWM_E4M3) with one fp32 scale per row;
  *    biases, norm weights, modulation vectors, residual streams are fp32.
  *  - there is NO CPU fallback: calling these without a Hopper (sm_90a) GPU fails.
+ *  - alignment (dwm_b200_linear, dwm_b200_conv): A / W / x / weight / out, bias, resid, gate,
+ *    blend_x and every peer_out are 16-byte aligned; the fp32 row pitches ldr, gate_ld and
+ *    ldx are multiples of 4 elements (16-byte rows), the 16-bit pitches multiples of 8.  The
+ *    epilogue reads these rows as float2 / float4 and the RESID rows are also prefetched by
+ *    bulk copies; a call that breaks a rule returns < 0 before anything is launched.
  */
 #ifndef DWM_B200_H_
 #define DWM_B200_H_
@@ -71,7 +76,9 @@ typedef struct dwm_linear_args {
   int64_t ldo;     /* row pitch of out, elements */
   /* item structure of the M rows: item(m) = m / rows_per_item (0 => one item).
    * 16-bit outputs go to row  item * out_item_stride + m % rows_per_item + out_row_offset
-   * (lets sample and context tokens of one view-frame land in one joint buffer). */
+   * (lets sample and context tokens of one view-frame land in one joint buffer).
+   * With rows_per_item > 0, 16-bit epilogues need out_item_stride >= rows_per_item (so that
+   * items never share output rows); fp32 outputs (RESID, F32) are never remapped. */
   int64_t rows_per_item;
   int64_t out_item_stride;
   int64_t out_row_offset;
@@ -306,7 +313,8 @@ typedef struct dwm_conv_args {
   const float* resid;
   int64_t ldr;
   /* resid_per_item != 0: `resid` holds ONE row per item of rows_per_item consecutive output
-   * pixels (ResnetBlock2D's `+ time_emb_proj(silu(temb))[:, :, None, None]`). */
+   * pixels (ResnetBlock2D's `+ time_emb_proj(silu(temb))[:, :, None, None]`).  resid,
+   * resid_per_item and blend_x need DWM_EPI_RESID; output rows are never remapped. */
   int resid_per_item;
   int64_t rows_per_item;
   /* optional AlphaBlender after the residual (DWM_EPI_RESID):

@@ -214,7 +214,8 @@ static int launch_conv(const dwm_conv_args* a, cudaStream_t stream) {
   p.out = a->out; p.ldo = a->ldo; p.bias = a->bias; p.act = a->act;
   p.resid = a->resid; p.ldr = a->ldr;
   p.resid_row_mod = a->resid_per_item ? -1 : 0;
-  p.rows_per_item = a->rows_per_item;
+  // rows_per_item only picks the residual row; the 16-bit store must not remap its rows by it
+  p.rows_per_item = EPI == DWM_EPI_RESID ? a->rows_per_item : 0;
   p.blend_x = a->blend_x; p.ldx = a->ldx; p.alpha = a->alpha; p.rows_per_batch = a->rows_per_batch;
   p.norm_regions = 2;
   p.n_peers = 0;
@@ -310,6 +311,20 @@ extern "C" int dwm_b200_conv(const dwm_conv_args* a, dwm_stream_t stream) {
               "dwm_b200_conv: alignment");
   const long long rows = a->nb * (a->tp - a->kt + 1) * a->h * a->w;
   DWM_REQUIRE(rows < (1ll << 31), "dwm_b200_conv: too many output pixels");
+  if (a->epilogue != DWM_EPI_RESID)
+    DWM_REQUIRE(!a->resid && !a->blend_x && !a->resid_per_item,
+                "dwm_b200_conv: resid, blend_x and resid_per_item need epilogue DWM_EPI_RESID");
+  if (a->blend_x) DWM_REQUIRE(a->alpha != nullptr, "dwm_b200_conv: blend_x without alpha");
+  if (a->resid_per_item)
+    DWM_REQUIRE(a->rows_per_item > 0, "dwm_b200_conv: resid_per_item needs rows_per_item > 0");
+  // the epilogue reads bias / resid / blend_x rows as float2 / float4
+  for (const void* p : {static_cast<const void*>(a->bias), static_cast<const void*>(a->resid),
+                        static_cast<const void*>(a->blend_x)})
+    DWM_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0,
+                "dwm_b200_conv: bias, resid, blend_x must be 16-byte aligned");
+  DWM_REQUIRE((!a->resid || a->ldr % 4 == 0) && (!a->blend_x || a->ldx % 4 == 0),
+              "dwm_b200_conv: ldr, ldx must be multiples of 4 (16-byte rows); got %lld %lld",
+              (long long)a->ldr, (long long)a->ldx);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (a->dtype == DWM_BF16) return conv_pick_epi<__nv_bfloat16>(a, s);
   if (a->dtype == DWM_F16) return conv_pick_epi<__half>(a, s);

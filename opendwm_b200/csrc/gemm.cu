@@ -274,6 +274,23 @@ extern "C" int dwm_b200_linear(const dwm_linear_args* a, dwm_stream_t stream) {
                 "dwm_b200_linear: peer_out needs a 16-bit epilogue");
   if (a->epilogue == DWM_EPI_RESID && a->blend_x)
     DWM_REQUIRE(a->alpha != nullptr, "dwm_b200_linear: blend_x without alpha");
+  // the epilogue reads bias / resid / gate / blend_x rows as float2 / float4, stores to the peers
+  // as 8-byte words at the offsets of `out`, and prefetches the RESID rows with cp.async.bulk
+  for (const void* p : {static_cast<const void*>(a->bias), static_cast<const void*>(a->resid),
+                        static_cast<const void*>(a->gate), static_cast<const void*>(a->blend_x)})
+    DWM_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0,
+                "dwm_b200_linear: bias, resid, gate, blend_x must be 16-byte aligned");
+  for (int i = 0; i < a->n_peer_out; ++i)
+    DWM_REQUIRE(a->peer_out[i] && (reinterpret_cast<uintptr_t>(a->peer_out[i]) & 15) == 0,
+                "dwm_b200_linear: peer_out[%d] must be a 16-byte aligned pointer", i);
+  DWM_REQUIRE((!a->resid || a->ldr % 4 == 0) && (!a->gate || a->gate_ld % 4 == 0) &&
+                  (!a->blend_x || a->ldx % 4 == 0),
+              "dwm_b200_linear: ldr, gate_ld, ldx must be multiples of 4 (16-byte rows); got %lld %lld %lld",
+              (long long)a->ldr, (long long)a->gate_ld, (long long)a->ldx);
+  if (a->rows_per_item > 0 && a->epilogue != DWM_EPI_RESID && a->epilogue != DWM_EPI_F32)
+    DWM_REQUIRE(a->out_item_stride >= a->rows_per_item,
+                "dwm_b200_linear: out_item_stride %lld < rows_per_item %lld would write several items "
+                "to the same output rows", (long long)a->out_item_stride, (long long)a->rows_per_item);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (g_gemm_2cta < 0) {
     const char* e = getenv("DWM_GEMM_2CTA");

@@ -65,6 +65,58 @@ def _rows2d(t, name):
 FP8 = torch.float8_e4m3fn
 
 
+def _cdiv(a, b):
+    return (a + b - 1) // b
+
+
+def _need(t, name, rows, cols):
+    """t must cover [rows, cols] (a 1-D t: cols elements)."""
+    if t is None:
+        return
+    have = (1, t.shape[0]) if t.dim() == 1 else (t.shape[0], t.shape[1])
+    if have[0] < rows or have[1] < cols:
+        raise ValueError("{} is {}, the epilogue addresses [{}, {}]".format(
+            name, list(t.shape), rows, cols))
+
+
+def _check_fp32_epilogue(rows, cols, bias, resid, resid_rows, blend_x, alpha, rows_per_batch):
+    """Extents of the fp32 operands every fused epilogue reads."""
+    _need(bias, "bias", 1, cols)
+    _need(resid, "resid", resid_rows, cols)
+    _need(blend_x, "blend_x", rows, cols)
+    if blend_x is not None and alpha is not None:
+        _need(alpha, "alpha", 1, _cdiv(rows, rows_per_batch) if rows_per_batch > 0 else 1)
+
+
+def _check_linear_extents(M, N, epilogue, out, bias, rows_per_item, out_item_stride,
+                          out_row_offset, resid, resid_row_mod, gate, blend_x, alpha,
+                          rows_per_batch):
+    """Every row the epilogue of dwm_b200_linear reads or writes lies inside its tensor."""
+    items = _cdiv(M, rows_per_item) if rows_per_item > 0 else 1
+    if epilogue in (_l.EPI_RESID, _l.EPI_F32):
+        out_rows = M
+    else:
+        if out_row_offset < 0:
+            raise ValueError("out_row_offset must be >= 0")
+        if rows_per_item > 0:
+            if out_item_stride < rows_per_item:
+                raise ValueError("out_item_stride {} < rows_per_item {}: items would share "
+                                 "output rows".format(out_item_stride, rows_per_item))
+            last = items - 1
+            out_rows = last * out_item_stride + (M - last * rows_per_item)
+        else:
+            out_rows = M
+        out_rows += out_row_offset
+    if out.shape[0] < out_rows:
+        raise ValueError("out has {} rows, the epilogue writes {}".format(out.shape[0], out_rows))
+    if resid_row_mod > 0:
+        resid_rows = min(resid_row_mod, M)
+    else:
+        resid_rows = items if resid_row_mod < 0 else M
+    _check_fp32_epilogue(M, N, bias, resid, resid_rows, blend_x, alpha, rows_per_batch)
+    _need(gate, "gate", items, N)
+
+
 def linear(a, w, bias=None, *, epilogue=_l.EPI_STORE, act=_l.ACT_NONE,
            out=None, rows_per_item=0, out_item_stride=0, out_row_offset=0,
            q_norm_weight=None, k_norm_weight=None, qk_region=0, eps=1e-6,
@@ -113,6 +165,9 @@ def linear(a, w, bias=None, *, epilogue=_l.EPI_STORE, act=_l.ACT_NONE,
         raise TypeError("out dtype {} != {}".format(out.dtype, want))
     if out.shape[1] < out_cols:
         raise ValueError("out has {} columns, need {}".format(out.shape[1], out_cols))
+    _check_linear_extents(M, N, epilogue, out, bias, rows_per_item, out_item_stride,
+                          out_row_offset, resid, resid_row_mod, gate, blend_x, alpha,
+                          rows_per_batch)
     args = _l.LinearArgs()
     args.M, args.N, args.K = M, N, K
     args.A, args.lda = a.data_ptr(), a.stride(0)
@@ -459,8 +514,15 @@ def conv(x, weight, bias=None, *, kernel, epilogue=_l.EPI_F32, act=_l.ACT_NONE,
     if out is None:
         out = torch.empty(rows, c_out, device=x.device, dtype=want)
     _rows2d(out, "out")
-    if out.dtype != want or out.shape[0] < rows:
+    if out.dtype != want or out.shape[0] < rows or out.shape[1] < c_out:
         raise TypeError("conv: bad out tensor")
+    if epilogue != _l.EPI_RESID and (resid is not None or blend_x is not None):
+        raise ValueError("conv: resid / blend_x need the RESID epilogue")
+    if resid_rows_per_item:
+        resid_rows = _cdiv(rows, resid_rows_per_item)
+    else:
+        resid_rows = rows
+    _check_fp32_epilogue(rows, c_out, bias, resid, resid_rows, blend_x, alpha, rows_per_batch)
     a = _l.ConvArgs()
     a.x, a.nb, a.tp, a.h, a.w, a.c_in = x.data_ptr(), nb, tp, h, w, c_in
     a.weight, a.kt, a.kh, a.kw, a.c_out = weight.data_ptr(), kt, kh, kw, c_out
