@@ -368,6 +368,35 @@ int dwm_b200_groupnorm_silu_e4m3(const float* x, int64_t nb, int64_t T, int64_t 
                                  int groups, const double* sums, float eps, const float* gamma,
                                  const float* beta, int apply_silu, void* out, int64_t out_T,
                                  int64_t out_t0, float* out_scale, dwm_stream_t stream);
+/* Frame-shard GroupNorm(+SiLU) of the temporal ResBlock convolutions: x holds T of a window's
+ * frames and `sums` (double [nb, groups, 2]) the statistics already summed over the window's
+ * `stat_frames` frames, so mean and variance use stat_frames*H*W*C/groups samples.  out is the
+ * shard's temporal-conv operand [nb, T + 2, H, W, C] with the local frames at 1 ... T.  Local
+ * frame 0 is also stored at frame prev_out_T - 1 of prev_out (the previous shard's operand
+ * [nb, prev_out_T, H, W, C]) and local frame T - 1 at frame 0 of next_out ([nb, next_out_T, ...]);
+ * the neighbours store their boundary frames into out the same way.  A NULL neighbour (first /
+ * last shard of the window) stores the own halo frame as zero, the conv's time padding.  The
+ * values are those of dwm_b200_spatialnorm_silu with zy = zb = NULL for the same sums. */
+int dwm_b200_groupnorm_silu_halo(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C,
+                                 int groups, const double* sums, int64_t stat_frames, float eps,
+                                 const float* gamma, const float* beta, int apply_silu, void* out,
+                                 void* prev_out, int64_t prev_out_T, void* next_out,
+                                 int64_t next_out_T, int dtype, dwm_stream_t stream);
+/* E4M3 frame-shard variant, pass 1: amax[n] (fp32 [nb]) = max |y| over the shard's frames of
+ * volume n, y as in dwm_b200_groupnorm_silu_halo.  Reduce it with MAX over the window's shards. */
+int dwm_b200_groupnorm_silu_e4m3_amax(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W,
+                                      int C, int groups, const double* sums, int64_t stat_frames,
+                                      float eps, const float* gamma, const float* beta,
+                                      int apply_silu, float* amax, dwm_stream_t stream);
+/* Pass 2: quantizes with the given (window-wide) amax exactly as dwm_b200_groupnorm_silu_e4m3
+ * does for that amax, writes out_scale[n] (may alias amax), and stores the frames and halo
+ * frames as dwm_b200_groupnorm_silu_halo does. */
+int dwm_b200_groupnorm_silu_e4m3_halo(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W,
+                                      int C, int groups, const double* sums, int64_t stat_frames,
+                                      float eps, const float* gamma, const float* beta,
+                                      int apply_silu, const float* amax, void* out, void* prev_out,
+                                      int64_t prev_out_T, void* next_out, int64_t next_out_T,
+                                      float* out_scale, dwm_stream_t stream);
 /* CogVideoXUpsample3D interpolation: nearest x2 in H, W and (compress_time) in T, where an
  * odd T > 1 keeps its first frame un-doubled in time; fp32 in, 16-bit out
  * [nb, T', 2H, 2W, C].  Also the F.interpolate(nearest, x2) of the UNet / AutoencoderKL

@@ -134,6 +134,12 @@ struct SnParams {
   int silu;
   void* out; int out_T, out_t0;
   float* scale;   // E4M3 output: [nb] amax bits (SN_AMAX pass), then the volume scale
+  int stat_T;     // frames the GroupNorm sums cover (T, or the whole window of a frame shard)
+  // HALO: frame-shard operand [nb, T + 2, H, W, C]; local frame 0 is also stored at frame
+  // prev_T - 1 of prev_out, the last local frame at frame 0 of next_out (both [nb, *_T, H, W, C]);
+  // without a neighbour the own halo frame is stored as zero
+  void* prev_out = nullptr; int prev_T = 0;
+  void* next_out = nullptr; int next_T = 0;
 };
 
 // What a spatialnorm_kernel pass does with each normalised float4: store it as 16 bit, only
@@ -151,7 +157,7 @@ enum { SN_STORE16 = 0, SN_AMAX = 1, SN_E4M3 = 2 };
 // are powers of two apart (always in the VAEs) and the frame map is a 64-entry shared table.
 // A version that spent ~10 integer divisions per float4 was far from DRAM-bound; this one is
 // a plain stream.
-template <typename T, int MODE = SN_STORE16>
+template <typename T, int MODE = SN_STORE16, bool HALO = false>
 __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, const int chunk) {
   // blockDim.x is a multiple of C/4 whenever C/4 <= 1024 (host side), `chunk` = blockDim.x * 16
   __shared__ float2 s_stat[64];
@@ -163,7 +169,7 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
   const int cg = p.C / p.G;
   const long long per_img = static_cast<long long>(p.T) * p.H * p.W * vec;
   if (threadIdx.x < p.G) {
-    const double cnt = static_cast<double>(cg) * p.T * p.H * p.W;
+    const double cnt = static_cast<double>(cg) * p.stat_T * p.H * p.W;
     const double s = p.sums[(static_cast<long long>(n) * p.G + threadIdx.x) * 2];
     const double ss = p.sums[(static_cast<long long>(n) * p.G + threadIdx.x) * 2 + 1];
     const double mean_d = s / cnt;
@@ -185,14 +191,42 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
   float amax = 0.f;
   float inv = 0.f;
   if constexpr (MODE == SN_E4M3) inv = e4m3_inv(__uint_as_float(reinterpret_cast<const uint32_t*>(p.scale)[n]));
-  auto emit = [&](long long o, const float4& v) {
+  auto store = [&](void* base, long long o, const float4& v) {
     if constexpr (MODE == SN_STORE16) {
       uint2 pk; pk.x = Cvt<T>::pack2(v.x, v.y); pk.y = Cvt<T>::pack2(v.z, v.w);
-      reinterpret_cast<uint2*>(p.out)[o] = pk;
-    } else if constexpr (MODE == SN_AMAX) {
+      reinterpret_cast<uint2*>(base)[o] = pk;
+    } else {
+      reinterpret_cast<uint32_t*>(base)[o] = e4m3x4(v.x, v.y, v.z, v.w, inv);
+    }
+  };
+  // the zero time padding, stored as bits (E4M3 through e4m3x4 left non-zero upper bytes)
+  auto store_zero = [&](long long o) {
+    if constexpr (MODE == SN_STORE16) reinterpret_cast<uint2*>(p.out)[o] = make_uint2(0u, 0u);
+    else reinterpret_cast<uint32_t*>(p.out)[o] = 0u;
+  };
+  // frame-to-frame distance of the output in float4 units (HALO offsets are whole frames)
+  const long long frame4 = static_cast<long long>(p.H) * p.W * vec;
+  auto emit = [&](long long o, const float4& v, int t) {
+    if constexpr (MODE == SN_AMAX) {
       amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
     } else {
-      reinterpret_cast<uint32_t*>(p.out)[o] = e4m3x4(v.x, v.y, v.z, v.w, inv);
+      store(p.out, o, v);
+      if constexpr (HALO) {
+        // o = ((n * out_T + out_t0 + t) * H*W + pixel) * vec + c4; re-based onto a neighbour's
+        // frame by whole frames
+        if (t == 0) {
+          if (p.prev_out)
+            store(p.prev_out, o + (static_cast<long long>(n) * (p.prev_T - p.out_T) + p.prev_T - 1 - p.out_t0) * frame4, v);
+          else
+            store_zero(o - frame4);
+        }
+        if (t == p.T - 1) {
+          if (p.next_out)
+            store(p.next_out, o + (static_cast<long long>(n) * (p.next_T - p.out_T) - p.out_t0 - t) * frame4, v);
+          else
+            store_zero(o + frame4);
+        }
+      }
     }
   };
   auto finish = [&]() {
@@ -251,7 +285,7 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
       }
       if (p.silu) { v.x = silu(v.x); v.y = silu(v.y); v.z = silu(v.z); v.w = silu(v.w); }
       const long long o = (((on + t) * p.H + h) * p.W + w) * vec + c4;
-      emit(o, v);
+      emit(o, v, t);
       w += pstep;
       while (w >= p.W) { w -= p.W; if (++h == p.H) { h = 0; ++t; } }
     }
@@ -296,15 +330,15 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
     }
     if (p.silu) { v.x = silu(v.x); v.y = silu(v.y); v.z = silu(v.z); v.w = silu(v.w); }
     const long long o = (((static_cast<long long>(n) * p.out_T + p.out_t0 + t) * p.H + h) * p.W + w) * vec + c4;
-    emit(o, v);
+    emit(o, v, t);
   }
   finish();
 }
 
-// amax (bits, left in scale[] by the SN_AMAX pass) -> E4M3 volume scale
-__global__ void e4m3_amax_to_scale_kernel(float* scale, int nb) {
+// amax (bits, left by the SN_AMAX pass; may alias scale) -> E4M3 volume scale
+__global__ void e4m3_amax_to_scale_kernel(const float* amax, float* scale, int nb) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n < nb) scale[n] = e4m3_scale(__uint_as_float(reinterpret_cast<const uint32_t*>(scale)[n]));
+  if (n < nb) scale[n] = e4m3_scale(__uint_as_float(reinterpret_cast<const uint32_t*>(amax)[n]));
 }
 
 // ---- nearest upsample x2 in space, optionally in time (CogVideoXUpsample3D rules) ----
@@ -382,7 +416,7 @@ extern "C" int dwm_b200_spatialnorm_silu(const float* x, int64_t nb, int64_t T, 
   p.x = x; p.nb = (int)nb; p.T = (int)T; p.H = (int)H; p.W = (int)W; p.C = C; p.G = groups;
   p.sums = sums; p.eps = eps; p.gamma = gamma; p.beta = beta; p.zy = zy; p.zb = zb;
   p.Tz = Tz; p.hz = hz; p.wz = wz; p.silu = apply_silu; p.out = out; p.out_T = (int)out_T; p.out_t0 = (int)out_t0;
-  p.scale = nullptr;
+  p.scale = nullptr; p.stat_T = (int)T;
   DWM_REQUIRE(groups <= 64 && nb <= 65535, "dwm_b200_spatialnorm_silu: groups <= 64 and nb <= 65535 required");
   const long long per_img = T * H * W * (C / 4);
   // block = the largest multiple of C/4 that fits 256 threads (or C/4 itself up to 1024), so a
@@ -415,7 +449,7 @@ extern "C" int dwm_b200_groupnorm_silu_e4m3(const float* x, int64_t nb, int64_t 
   p.x = x; p.nb = (int)nb; p.T = (int)T; p.H = (int)H; p.W = (int)W; p.C = C; p.G = groups;
   p.sums = sums; p.eps = eps; p.gamma = gamma; p.beta = beta; p.zy = nullptr; p.zb = nullptr;
   p.Tz = p.hz = p.wz = 0; p.silu = apply_silu; p.out = out; p.out_T = (int)out_T; p.out_t0 = (int)out_t0;
-  p.scale = out_scale;
+  p.scale = out_scale; p.stat_T = (int)T;
   const long long per_img = T * H * W * (C / 4);
   const int vec = C / 4;
   int threads = 256;
@@ -426,7 +460,112 @@ extern "C" int dwm_b200_groupnorm_silu_e4m3(const float* x, int64_t nb, int64_t 
   DWM_CHECK_CUDA(cudaMemsetAsync(out_scale, 0, sizeof(float) * nb, s));
   spatialnorm_kernel<__nv_fp8_e4m3, SN_AMAX><<<grid, threads, 0, s>>>(p, chunk);
   spatialnorm_kernel<__nv_fp8_e4m3, SN_E4M3><<<grid, threads, 0, s>>>(p, chunk);
-  e4m3_amax_to_scale_kernel<<<static_cast<unsigned>((nb + 127) / 128), 128, 0, s>>>(out_scale, (int)nb);
+  e4m3_amax_to_scale_kernel<<<static_cast<unsigned>((nb + 127) / 128), 128, 0, s>>>(out_scale, out_scale, (int)nb);
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- frame-shard variants: statistics of the whole window, halo frames into the neighbours ----
+namespace {
+
+const char* gn_shard_check(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C, int groups,
+                           const double* sums, int64_t stat_frames, const float* gamma, const float* beta,
+                           int c_align) {
+  if (!x || !sums || !gamma || !beta) return "null pointer";
+  if (nb <= 0 || T <= 0 || H <= 0 || W <= 0 || nb > 65535) return "bad shape (need nb <= 65535)";
+  if (C % c_align || groups <= 0 || groups > 64 || C % groups) return "bad C / groups";
+  if (stat_frames < T) return "stat_frames < T";
+  return nullptr;
+}
+
+SnParams gn_shard_params(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C, int groups,
+                         const double* sums, int64_t stat_frames, float eps, const float* gamma,
+                         const float* beta, int apply_silu) {
+  SnParams p;
+  p.x = x; p.nb = (int)nb; p.T = (int)T; p.H = (int)H; p.W = (int)W; p.C = C; p.G = groups;
+  p.sums = sums; p.eps = eps; p.gamma = gamma; p.beta = beta; p.zy = nullptr; p.zb = nullptr;
+  p.Tz = p.hz = p.wz = 0; p.silu = apply_silu; p.out = nullptr; p.out_T = (int)T + 2; p.out_t0 = 1;
+  p.scale = nullptr; p.stat_T = (int)stat_frames;
+  return p;
+}
+
+// the launch shape of dwm_b200_spatialnorm_silu
+void gn_launch_shape(const SnParams& p, int* threads, int* chunk, dim3* grid) {
+  const int vec = p.C / 4;
+  *threads = 256;
+  if (vec <= 1024) *threads = vec <= 256 ? (256 / vec) * vec : vec;
+  *chunk = *threads * 16;
+  const long long per_img = static_cast<long long>(p.T) * p.H * p.W * vec;
+  *grid = dim3(static_cast<unsigned>((per_img + *chunk - 1) / *chunk), static_cast<unsigned>(p.nb));
+}
+
+const char* gn_halo_check(void* out, void* prev_out, int64_t prev_out_T, void* next_out, int64_t next_out_T) {
+  if (!out) return "null out";
+  if ((prev_out && prev_out_T < 3) || (next_out && next_out_T < 3)) return "neighbour buffers hold >= 3 frames";
+  return nullptr;
+}
+
+}  // namespace
+
+extern "C" int dwm_b200_groupnorm_silu_halo(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C,
+                                            int groups, const double* sums, int64_t stat_frames, float eps,
+                                            const float* gamma, const float* beta, int apply_silu, void* out,
+                                            void* prev_out, int64_t prev_out_T, void* next_out,
+                                            int64_t next_out_T, int dtype, dwm_stream_t stream) {
+  const char* bad = gn_shard_check(x, nb, T, H, W, C, groups, sums, stat_frames, gamma, beta, 4);
+  if (!bad) bad = gn_halo_check(out, prev_out, prev_out_T, next_out, next_out_T);
+  DWM_REQUIRE(!bad, "dwm_b200_groupnorm_silu_halo: %s", bad);
+  SnParams p = gn_shard_params(x, nb, T, H, W, C, groups, sums, stat_frames, eps, gamma, beta, apply_silu);
+  p.out = out; p.prev_out = prev_out; p.prev_T = (int)prev_out_T; p.next_out = next_out; p.next_T = (int)next_out_T;
+  int threads, chunk;
+  dim3 grid;
+  gn_launch_shape(p, &threads, &chunk, &grid);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (dtype == DWM_BF16) spatialnorm_kernel<__nv_bfloat16, SN_STORE16, true><<<grid, threads, 0, s>>>(p, chunk);
+  else if (dtype == DWM_F16) spatialnorm_kernel<__half, SN_STORE16, true><<<grid, threads, 0, s>>>(p, chunk);
+  else { set_last_error("dwm_b200_groupnorm_silu_halo: bad dtype"); return -1; }
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dwm_b200_groupnorm_silu_e4m3_amax(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W,
+                                                 int C, int groups, const double* sums, int64_t stat_frames,
+                                                 float eps, const float* gamma, const float* beta, int apply_silu,
+                                                 float* amax, dwm_stream_t stream) {
+  const char* bad = gn_shard_check(x, nb, T, H, W, C, groups, sums, stat_frames, gamma, beta, 16);
+  if (!bad && !amax) bad = "null amax";
+  DWM_REQUIRE(!bad, "dwm_b200_groupnorm_silu_e4m3_amax: %s", bad);
+  SnParams p = gn_shard_params(x, nb, T, H, W, C, groups, sums, stat_frames, eps, gamma, beta, apply_silu);
+  p.scale = amax;
+  int threads, chunk;
+  dim3 grid;
+  gn_launch_shape(p, &threads, &chunk, &grid);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  DWM_CHECK_CUDA(cudaMemsetAsync(amax, 0, sizeof(float) * nb, s));
+  spatialnorm_kernel<__nv_fp8_e4m3, SN_AMAX><<<grid, threads, 0, s>>>(p, chunk);
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dwm_b200_groupnorm_silu_e4m3_halo(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W,
+                                                 int C, int groups, const double* sums, int64_t stat_frames,
+                                                 float eps, const float* gamma, const float* beta, int apply_silu,
+                                                 const float* amax, void* out, void* prev_out, int64_t prev_out_T,
+                                                 void* next_out, int64_t next_out_T, float* out_scale,
+                                                 dwm_stream_t stream) {
+  const char* bad = gn_shard_check(x, nb, T, H, W, C, groups, sums, stat_frames, gamma, beta, 16);
+  if (!bad) bad = gn_halo_check(out, prev_out, prev_out_T, next_out, next_out_T);
+  if (!bad && (!amax || !out_scale)) bad = "null amax / out_scale";
+  DWM_REQUIRE(!bad, "dwm_b200_groupnorm_silu_e4m3_halo: %s", bad);
+  SnParams p = gn_shard_params(x, nb, T, H, W, C, groups, sums, stat_frames, eps, gamma, beta, apply_silu);
+  p.out = out; p.prev_out = prev_out; p.prev_T = (int)prev_out_T; p.next_out = next_out; p.next_T = (int)next_out_T;
+  p.scale = const_cast<float*>(amax);     // SN_E4M3 only reads it
+  int threads, chunk;
+  dim3 grid;
+  gn_launch_shape(p, &threads, &chunk, &grid);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  spatialnorm_kernel<__nv_fp8_e4m3, SN_E4M3, true><<<grid, threads, 0, s>>>(p, chunk);
+  e4m3_amax_to_scale_kernel<<<static_cast<unsigned>((nb + 127) / 128), 128, 0, s>>>(amax, out_scale, (int)nb);
   DWM_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -600,6 +600,81 @@ def groupnorm_silu_e4m3(x, sums, gamma, beta, out, scale, *, groups, eps=1e-6, o
     return out, scale
 
 
+def _halo_args(x, out, prev_out, next_out, dtype):
+    """Checks a frame shard's operand out [nb, T + 2, H, W, C] and its neighbours' operands
+    (None at the ends of the window) -> (prev ptr, prev frames, next ptr, next frames)."""
+    _f32(x, "x")
+    if x.dim() != 5 or not x.is_contiguous():
+        raise ValueError("x must be contiguous [nb, T, H, W, C]")
+    nb, T = x.shape[:2]
+    args = []
+    for name, t, want_T in (("out", out, T + 2), ("prev_out", prev_out, None),
+                            ("next_out", next_out, None)):
+        if t is None and name != "out":
+            args += [None, 0]
+            continue
+        if t.dtype != dtype or t.dim() != 5 or not t.is_contiguous() or t.shape[0] != nb or \
+                t.shape[2:] != x.shape[2:] or t.shape[1] < 3 or \
+                (want_T is not None and t.shape[1] != want_T):
+            raise ValueError("{} must be contiguous {} [nb, {}, H, W, C]".format(
+                name, dtype, "T + 2" if want_T else "frames + 2"))
+        if name != "out":
+            args += [t.data_ptr(), t.shape[1]]
+    return args
+
+
+def groupnorm_silu_halo(x, sums, gamma, beta, out, *, groups, stat_frames, prev_out=None,
+                        next_out=None, eps=1e-6, silu=True):
+    """GroupNorm(+SiLU) of a frame shard x fp32 [nb,T,H,W,C] with statistics `sums` summed over
+    the window's `stat_frames` frames, into the shard's 16-bit temporal-conv operand
+    out [nb,T+2,H,W,C] (local frames at 1..T); the boundary frames are also stored into the
+    neighbours' operands prev_out / next_out, a missing neighbour leaves a zero halo frame."""
+    halo = _halo_args(x, out, prev_out, next_out, out.dtype)
+    nb, T, H, W, C = x.shape
+    _l.check(_l.load().dwm_b200_groupnorm_silu_halo(
+        x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), stat_frames, eps,
+        _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(), int(silu),
+        out.data_ptr(), *halo, _dt(out), _stream()), "dwm_b200_groupnorm_silu_halo")
+    return out
+
+
+def groupnorm_silu_e4m3_amax(x, sums, gamma, beta, amax, *, groups, stat_frames, eps=1e-6,
+                             silu=True):
+    """First E4M3 frame-shard pass: amax fp32 [nb] of the shard's GroupNorm(+SiLU) output, to be
+    reduced with MAX over the window's shards before `groupnorm_silu_e4m3_halo`."""
+    _f32(x, "x")
+    if x.dim() != 5 or not x.is_contiguous():
+        raise ValueError("x must be contiguous [nb, T, H, W, C]")
+    nb, T, H, W, C = x.shape
+    _f32(amax, "amax")
+    if amax.numel() != nb or not amax.is_contiguous():
+        raise ValueError("amax must be fp32 [nb]")
+    _l.check(_l.load().dwm_b200_groupnorm_silu_e4m3_amax(
+        x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), stat_frames, eps,
+        _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(), int(silu),
+        amax.data_ptr(), _stream()), "dwm_b200_groupnorm_silu_e4m3_amax")
+    return amax
+
+
+def groupnorm_silu_e4m3_halo(x, sums, gamma, beta, amax, out, scale, *, groups, stat_frames,
+                             prev_out=None, next_out=None, eps=1e-6, silu=True):
+    """Second E4M3 frame-shard pass: quantizes with the window's amax [nb] into
+    out float8_e4m3fn [nb,T+2,H,W,C] and scale [nb] (the bytes and scales groupnorm_silu_e4m3
+    gives for that amax), halo frames as in `groupnorm_silu_halo`."""
+    halo = _halo_args(x, out, prev_out, next_out, FP8)
+    nb, T, H, W, C = x.shape
+    for t, name in ((amax, "amax"), (scale, "scale")):
+        _f32(t, name)
+        if t.numel() != nb or not t.is_contiguous():
+            raise ValueError("{} must be fp32 [nb]".format(name))
+    _l.check(_l.load().dwm_b200_groupnorm_silu_e4m3_halo(
+        x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), stat_frames, eps,
+        _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(), int(silu),
+        amax.data_ptr(), out.data_ptr(), *halo, scale.data_ptr(), _stream()),
+        "dwm_b200_groupnorm_silu_e4m3_halo")
+    return out, scale
+
+
 def upsample_nearest(x, compress_time, dtype):
     _f32(x, "x")
     nb, T, H, W, C = x.shape

@@ -110,6 +110,48 @@ class ShardPlan:
                 parts[r, :, :self.counts[r]]
         return _Done() if async_op else None
 
+    def reduce_group_sums(self, sums: torch.Tensor):
+        """In place: the fp64 GroupNorm statistics [nb, groups, 2] (sum, sum of squares) of the
+        local frames -> those of the whole window (all-reduce SUM over the frame group)."""
+        if self.t_ways > 1:
+            dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=self.t_group)
+        return sums
+
+    def reduce_amax(self, amax: torch.Tensor):
+        """In place: per-volume amax of the local frames -> of the whole window (MAX)."""
+        if self.t_ways > 1:
+            dist.all_reduce(amax, op=dist.ReduceOp.MAX, group=self.t_group)
+        return amax
+
+    def exchange_halo(self, buf: torch.Tensor):
+        """Point-to-point halo exchange of a frame shard's temporal-conv operand buf
+        [nb, T_loc + 2, ...] (local frames at 1 ... T_loc): frame 0 receives the previous
+        shard's last frame, frame T_loc + 1 the next shard's first frame.  The window's first
+        and last frames keep what buf holds there (the zero time padding).  The fallback of the
+        fused halo stores (`PeerHalo`); gloo moves host copies (it has no device send / recv)."""
+        if self.t_ways == 1:
+            return buf
+        raw = buf.view(torch.uint8) if buf.element_size() == 1 else buf
+        host = dist.get_backend(self.t_group) == "gloo" and raw.is_cuda
+        base = self.cfg_rank * self.t_ways
+        ops, recvs = [], []
+        for nbr, send_t, recv_t in ((self.t_rank - 1, 1, 0),
+                                    (self.t_rank + 1, self.T_loc, self.T_loc + 1)):
+            if not 0 <= nbr < self.t_ways:
+                continue
+            snd = raw[:, send_t].contiguous()
+            rcv = torch.empty_like(snd)
+            if host:
+                snd, rcv = snd.cpu(), rcv.cpu()
+            ops += [dist.P2POp(dist.isend, snd, base + nbr, self.t_group),
+                    dist.P2POp(dist.irecv, rcv, base + nbr, self.t_group)]
+            recvs.append((recv_t, rcv))
+        for w in dist.batch_isend_irecv(ops):
+            w.wait()
+        for t, rcv in recvs:
+            raw[:, t].copy_(rcv)
+        return buf
+
     def gather_cfg_tokens(self, tokens: torch.Tensor, out: torch.Tensor):
         """out = [uncond tokens ; cond tokens] on both ranks of the CFG pair."""
         return dist.all_gather_into_tensor(out, tokens, group=self.cfg_group)
@@ -195,3 +237,54 @@ class PeerKV:
         peers = [int(hdl.buffer_ptrs[q]) for q in range(self.plan.t_ways)
                  if q != self.plan.t_rank]
         return buf, peers, hdl
+
+
+class PeerHalo:
+    """Temporal-conv operands of a frame group in symmetric (peer-mapped) memory.
+
+    A frame shard's GroupNorm(+SiLU) kernel writes its operand [nb, T_loc + 2, H, W, C] and
+    stores its first / last frame straight into the previous / next shard's operand
+    (`ops.groupnorm_silu_halo`), so the halo frames cross NVLink inside the kernel; one group
+    barrier then publishes them to the conv.  The buffers are sized once for the largest
+    operand of the forward (`nbytes`) and every temporal ResBlock level views them at its own
+    shape.  Two buffers alternate between consecutive temporal convs, and that is enough with
+    one barrier per conv: a rank writes buffer b for conv k + 2 (its own frames and its
+    neighbours' halo frames) only after it passed the barrier of conv k + 1, which every peer
+    reaches only after its conv k, the last reader of buffer b, ran (the barrier is ordered on
+    the stream after it)."""
+
+    def __init__(self, plan: ShardPlan, nbytes: int, device):
+        import torch.distributed._symmetric_memory as symm_mem
+        self.plan, self.nbytes = plan, nbytes
+        self.bufs, self.handles = [], []
+        for _ in range(2):
+            t = symm_mem.empty(nbytes, dtype=torch.uint8, device=device)
+            self.bufs.append(t)
+            self.handles.append(symm_mem.rendezvous(t, plan.t_group))
+        self.turn = 0
+
+    def next(self, shape, dtype):
+        """(own operand, previous shard's operand or None, next shard's or None, handle): views
+        of the next buffer at `shape` [nb, T_loc + 2, ...] of this rank and at the neighbours'
+        frame counts."""
+        b = self.turn
+        self.turn ^= 1
+        hdl, plan = self.handles[b], self.plan
+        per_frame = shape[0], shape[2:]
+
+        def view(q):
+            size = (per_frame[0], plan.counts[q] + 2) + tuple(per_frame[1])
+            n = 1
+            for s in size:
+                n *= s
+            if n * dtype.itemsize > self.nbytes:
+                raise ValueError("PeerHalo holds {} bytes, {} needs more".format(
+                    self.nbytes, size))
+            if q == plan.t_rank:
+                return self.bufs[b][:n * dtype.itemsize].view(dtype).view(size)
+            return hdl.get_buffer(q, size, dtype)
+        if shape[1] != plan.T_loc + 2:
+            raise ValueError("operand frames {} != T_loc + 2".format(shape[1]))
+        prev = view(plan.t_rank - 1) if plan.t_rank > 0 else None
+        nxt = view(plan.t_rank + 1) if plan.t_rank + 1 < plan.t_ways else None
+        return view(plan.t_rank), prev, nxt, hdl

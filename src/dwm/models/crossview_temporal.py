@@ -112,6 +112,73 @@ class AlphaBlender(torch.nn.Module):
             if a.numel() == 1 else a.flatten().contiguous()
 
 
+def sharded_temporal_qkv_attend(plan, kind, B, T_loc, V, Hp, Wp, D, heads, q_loc, peer_kv=None,
+                                kv_loc=None, kv_all=None, eps=1e-5):
+    """`VTSelfAttentionBlock.run`'s qkv_attend for frame-sharded temporal attention (kind
+    "full", "rowwise" or "pointwise"; even or uneven frame shards of a ShardPlan): K,V of the
+    local frames are projected (+RMSNorm) straight into the gathered buffer, which keeps the
+    UNSHARDED row layout (b, t, v, s) on every rank — through the GEMM epilogue's item row
+    mapping into local AND peer memory (fused scatter over NVLink, `peer_kv` a PeerKV whose
+    buffers hold at least B*T*V*S x 2D), or through an all-gather (kv_loc, kv_all) — while
+    the Q projection runs into q_loc; then every local query frame attends to all T frames
+    with the single-GPU key addressing."""
+    S, T = Hp * Wp, plan.T
+    # local rows -> rows of the unsharded layout: item = batch entry
+    remap = dict(rows_per_item=T_loc * V * S, out_item_stride=T * V * S,
+                 out_row_offset=plan.t_offset * V * S)
+
+    def project(p, a, w, nw, out, peer_out=None, **kw):
+        if p["qk_norm"]:
+            gemm(a, w, epilogue=_lib.EPI_QKNORM, out=out,
+                 q_norm_weight=nw, qk_region=D, qk_norm_regions=1,
+                 eps=eps, peer_out=peer_out, **kw)
+        else:
+            gemm(a, w, out=out, peer_out=peer_out, **kw)
+
+    def attend(kv_all, out):
+        if kind == "full":         # (b v) (t hw)
+            _ops.attention(
+                q_loc, out, D=D, heads=heads, group_dims=[B, V],
+                group_strides=[T_loc * V * S, S], seq=T_loc * S, inner=S,
+                stride_outer=V * S, stride_inner=1, kv=kv_all, k_col=0, v_col=D,
+                kv_group_strides=[T * V * S, S], seq_kv=T * S, inner_kv=S,
+                kv_stride_outer=V * S, kv_stride_inner=1)
+        elif kind == "rowwise":    # (b v h) (t w)
+            _ops.attention(
+                q_loc, out, D=D, heads=heads, group_dims=[B, V, Hp],
+                group_strides=[T_loc * V * S, S, Wp], seq=T_loc * Wp, inner=Wp,
+                stride_outer=V * S, stride_inner=1, kv=kv_all, k_col=0, v_col=D,
+                kv_group_strides=[T * V * S, S, Wp], seq_kv=T * Wp, inner_kv=Wp,
+                kv_stride_outer=V * S, kv_stride_inner=1)
+        else:                      # pointwise: (b v hw) t
+            _ops.attention(
+                q_loc, out, D=D, heads=heads, group_dims=[B, V * S],
+                group_strides=[T_loc * V * S, 1], seq=T_loc, inner=1,
+                stride_outer=V * S, stride_inner=0, kv=kv_all, k_col=0, v_col=D,
+                kv_group_strides=[T * V * S, 1], seq_kv=T, inner_kv=1,
+                kv_stride_outer=V * S, kv_stride_inner=0)
+
+    def qkv_attend(p, a, out):
+        q, kv = p["qkv"].rows(0, D), p["qkv"].rows(D, 3 * D)
+        if peer_kv is not None:
+            # fused: the K,V GEMM epilogue scatters its tiles into every peer's
+            # gathered buffer over NVLink; one group barrier publishes them
+            kv_full, peers, hdl = peer_kv.next()
+            # the leading rows at this block's width (peers address their buffers the same way)
+            kv_full = kv_full.view(-1)[:B * T * V * S * 2 * D].view(B * T * V * S, 2 * D)
+            project(p, a, kv, p.get("nk"), kv_full, peers, **remap)
+            project(p, a, q, p.get("nq"), q_loc)
+            hdl.barrier(channel=0)
+        else:
+            kv_full = kv_all
+            project(p, a, kv, p.get("nk"), kv_loc)
+            work = plan.gather_frames_kv(kv_loc, kv_full, batch=B, async_op=True)
+            project(p, a, q, p.get("nq"), q_loc)
+            work.wait()
+        attend(kv_full, out)
+    return qkv_attend
+
+
 class VTSelfAttentionBlock(torch.nn.Module):
     """LN -> GEGLU-FF + res ; LN -> MHSA(+qk RMSNorm) + res ; LN -> GEGLU-FF + res
     (reference crossview_temporal.py:536-582), executed as 3 LayerNorm launches,

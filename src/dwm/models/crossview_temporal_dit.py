@@ -31,7 +31,8 @@ from opendwm_b200 import ops as _ops
 from .. import _compat
 from . import adapters as _adapters
 from .crossview_temporal import (
-    AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward)
+    AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward,
+    sharded_temporal_qkv_attend)
 from .packing import (
     FP8, Operand, fp32, fp8_bytes_saved, gemm, layernorm, pack_linear, requantize)
 
@@ -614,12 +615,8 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         return attend
 
     def _temporal_qkv_attend_sharded(self, B, T_loc, V, Hp, Wp, ws):
-        """Frame-sharded temporal attention (any temporal_attention_type, even or uneven frame
-        shards): K,V of the local frames are projected (+RMSNorm) straight into the gathered
-        buffer, which keeps the UNSHARDED row layout (b, t, v, s) on every rank — through the
-        GEMM epilogue's item row mapping into local AND peer memory (fused scatter over
-        NVLink), or through an all-gather — while the Q projection runs; then every local
-        query frame attends to all T frames with the single-GPU key addressing."""
+        """Frame-sharded temporal attention (`sharded_temporal_qkv_attend`) with its buffers
+        kept in the step workspace for the input geometry."""
         plan = self.shard
         S, D, heads = Hp * Wp, self.inner_dim, self.heads
         T = plan.T
@@ -636,61 +633,9 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
             else:
                 ws["kv_loc"] = torch.empty(rows, 2 * D, device=dev, dtype=dt)
                 ws["kv_all"] = torch.empty(rows_full, 2 * D, device=dev, dtype=dt)
-        q_loc, peer_kv = ws["q_loc"], ws["peer_kv"]
-        eps = 1e-5
-        kind = self.temporal_attention_type
-        # local rows -> rows of the unsharded layout: item = batch entry
-        remap = dict(rows_per_item=T_loc * V * S, out_item_stride=T * V * S,
-                     out_row_offset=plan.t_offset * V * S)
-
-        def project(p, a, w, nw, out, peer_out=None, **kw):
-            if p["qk_norm"]:
-                gemm(a, w, epilogue=_lib.EPI_QKNORM, out=out,
-                     q_norm_weight=nw, qk_region=D, qk_norm_regions=1,
-                     eps=eps, peer_out=peer_out, **kw)
-            else:
-                gemm(a, w, out=out, peer_out=peer_out, **kw)
-
-        def attend(kv_all, out):
-            if kind == "full":         # (b v) (t hw)
-                _ops.attention(
-                    q_loc, out, D=D, heads=heads, group_dims=[B, V],
-                    group_strides=[T_loc * V * S, S], seq=T_loc * S, inner=S,
-                    stride_outer=V * S, stride_inner=1, kv=kv_all, k_col=0, v_col=D,
-                    kv_group_strides=[T * V * S, S], seq_kv=T * S, inner_kv=S,
-                    kv_stride_outer=V * S, kv_stride_inner=1)
-            elif kind == "rowwise":    # (b v h) (t w)
-                _ops.attention(
-                    q_loc, out, D=D, heads=heads, group_dims=[B, V, Hp],
-                    group_strides=[T_loc * V * S, S, Wp], seq=T_loc * Wp, inner=Wp,
-                    stride_outer=V * S, stride_inner=1, kv=kv_all, k_col=0, v_col=D,
-                    kv_group_strides=[T * V * S, S, Wp], seq_kv=T * Wp, inner_kv=Wp,
-                    kv_stride_outer=V * S, kv_stride_inner=1)
-            else:                      # pointwise: (b v hw) t
-                _ops.attention(
-                    q_loc, out, D=D, heads=heads, group_dims=[B, V * S],
-                    group_strides=[T_loc * V * S, 1], seq=T_loc, inner=1,
-                    stride_outer=V * S, stride_inner=0, kv=kv_all, k_col=0, v_col=D,
-                    kv_group_strides=[T * V * S, 1], seq_kv=T, inner_kv=1,
-                    kv_stride_outer=V * S, kv_stride_inner=0)
-
-        def qkv_attend(p, a, out):
-            q, kv = p["qkv"].rows(0, D), p["qkv"].rows(D, 3 * D)
-            if peer_kv is not None:
-                # fused: the K,V GEMM epilogue scatters its tiles into every peer's
-                # gathered buffer over NVLink; one group barrier publishes them
-                kv_all, peers, hdl = peer_kv.next()
-                project(p, a, kv, p.get("nk"), kv_all, peers, **remap)
-                project(p, a, q, p.get("nq"), q_loc)
-                hdl.barrier(channel=0)
-            else:
-                kv_loc, kv_all = ws["kv_loc"], ws["kv_all"]
-                project(p, a, kv, p.get("nk"), kv_loc)
-                work = plan.gather_frames_kv(kv_loc, kv_all, batch=B, async_op=True)
-                project(p, a, q, p.get("nq"), q_loc)
-                work.wait()
-            attend(kv_all, out)
-        return qkv_attend
+        return sharded_temporal_qkv_attend(
+            plan, self.temporal_attention_type, B, T_loc, V, Hp, Wp, D, heads, ws["q_loc"],
+            peer_kv=ws["peer_kv"], kv_loc=ws.get("kv_loc"), kv_all=ws.get("kv_all"))
 
     # -- one JointTransformerBlock ----------------------------------------------------------
     def _joint_block(self, b, ws, N, S, L, residual):

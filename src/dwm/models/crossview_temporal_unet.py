@@ -22,7 +22,8 @@ from opendwm_b200 import ops as _ops
 from .. import _compat
 from . import adapters as _adapters
 from .crossview_temporal import (
-    AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward)
+    AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward,
+    sharded_temporal_qkv_attend)
 from .packing import (
     FP8, Operand, conv, gemm, layernorm, pack_conv, pack_linear, pack_norm, requantize)
 
@@ -258,6 +259,10 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         self._cond_key = None
         self._cond = None
         self._ws8, self._ws8_key = {}, None
+        # opendwm_b200.sharding.ShardPlan: with t_ways > 1, `sample` holds the plan's frame
+        # shard of the window; temporal ResBlocks and temporal attention exchange across it
+        self.shard = None
+        self._peer, self._peer_key = None, None
 
     # -- plumbing ---------------------------------------------------------------------------
     def enable_gradient_checkpointing(self):
@@ -408,6 +413,64 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         return _ops.spatialnorm_silu(x5, sums, g[0], g[1], out, groups=32, eps=g[2],
                                      out_t0=out_t0, silu=True)
 
+    def _frame_sharded(self):
+        return self.shard is not None and self.shard.t_ways > 1
+
+    def _peer_buffers(self, geo, H, W):
+        """Symmetric-memory K,V (PeerKV) and temporal-conv operand (PeerHalo) buffers of the
+        frame group, sized once per input geometry for the largest level (channels x pixels)
+        and shared by all temporal blocks in forward order: creating them is collective, so it
+        must not happen per block or per step.  (None, None) with DWM_PEER_SCATTER=0."""
+        plan = self.shard
+        dt = self._pk["dtype"]
+        key = (id(plan), geo, H, W, dt)
+        if self._peer_key != key:
+            self._peer, self._peer_key = (None, None), key
+            if plan.use_peer_scatter:
+                from opendwm_b200.sharding import PeerHalo, PeerKV
+                B, _, V = geo
+                widest, h, w = 0, H, W
+                for c in self.config["block_out_channels"]:
+                    widest = max(widest, c * h * w)
+                    h, w = (h + 1) // 2, (w + 1) // 2
+                dev = self.conv_in.weight.device
+                self._peer = (
+                    PeerKV(plan, B * plan.T * V * widest, 2, dt, dev),
+                    PeerHalo(plan, B * V * (max(plan.counts) + 2) * widest * dt.itemsize, dev))
+        return self._peer
+
+    def _norm_act_shard(self, x5, g):
+        """`_norm_act` of a frame shard x5 [nb, T_loc, H, W, C] into the temporal-conv operand
+        [nb, T_loc + 2, H, W, C]: GroupNorm statistics (and in E4M3 the volume amax) reduced
+        over the window's frames, frames 0 and T_loc + 1 the neighbour shards' boundary frames
+        (zero at the window's ends)."""
+        plan = self.shard
+        nb, T, H, W, C = x5.shape
+        fp8 = self._pk["fp8"]
+        dt = FP8 if fp8 else self._pk["dtype"]
+        sums = plan.reduce_group_sums(_ops.groupnorm_stats(x5, 32))
+        halo = self._peer[1]
+        if halo is not None:       # fused: the kernel stores the halo frames into the peers
+            out, prev, nxt, hdl = halo.next((nb, T + 2, H, W, C), dt)
+        else:
+            out, prev, nxt, hdl = torch.empty(nb, T + 2, H, W, C, device=x5.device,
+                                              dtype=dt), None, None, None
+        kw = dict(groups=32, stat_frames=plan.T, prev_out=prev, next_out=nxt, eps=g[2])
+        if fp8:
+            amax = torch.empty(nb, device=x5.device, dtype=torch.float32)
+            _ops.groupnorm_silu_e4m3_amax(x5, sums, g[0], g[1], amax, groups=32,
+                                          stat_frames=plan.T, eps=g[2])
+            plan.reduce_amax(amax)
+            res = Operand(*_ops.groupnorm_silu_e4m3_halo(
+                x5, sums, g[0], g[1], amax, out, torch.empty_like(amax), **kw))
+        else:
+            res = _ops.groupnorm_silu_halo(x5, sums, g[0], g[1], out, **kw)
+        if hdl is not None:
+            hdl.barrier(channel=0)
+        else:
+            plan.exchange_halo(out)
+        return res
+
     def _resblock(self, p, h, N, H, W, temb_all, geo, dis_t, alpha_mod):
         S = H * W
 
@@ -441,6 +504,8 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             .reshape(B * V * T, n).contiguous()
 
         def norm_act(t5, g):    # T + 2 frames, zero at both ends; E4M3: one scale per (b v)
+            if self._frame_sharded():     # ends: the neighbour shards' frames
+                return self._norm_act_shard(t5, g)
             return self._norm_act(t5, g, out_T=T + 2, out_t0=1)
         h1 = conv(norm_act(x5, p["n1"]), p["c1"], kernel=(3, 1, 1),
                   epilogue=_lib.EPI_RESID, resid=temb_p, resid_rows_per_item=S)
@@ -492,10 +557,26 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                 tabs["v"] = self._index_table(V, p["vpe"], tm.in_channels, dev, dt)[item_v]\
                     .contiguous()
             if "tpe" in p:
-                tabs["t"] = self._index_table(T, p["tpe"], tm.in_channels, dev, dt)[item_t]\
-                    .contiguous()
+                if self._frame_sharded():     # frame index within the whole window
+                    tab = self._index_table(self.shard.T, p["tpe"], tm.in_channels, dev, dt)
+                    item_t = item_t + self.shard.t_offset
+                else:
+                    tab = self._index_table(T, p["tpe"], tm.in_channels, dev, dt)
+                tabs["t"] = tab[item_t].contiguous()
             cd[key] = tabs
         tabs = cd[key]
+        tp_sharded = None
+        if "tp" in p and self._frame_sharded():
+            plan, rows = self.shard, N * S
+            peer_kv = self._peer[0]
+            kv_loc = kv_all = None
+            if peer_kv is None:
+                kv_loc = torch.empty(rows, 2 * inner, device=dev, dtype=dt)
+                kv_all = torch.empty(B * plan.T * V * S, 2 * inner, device=dev, dtype=dt)
+            tp_sharded = sharded_temporal_qkv_attend(
+                plan, "rowwise" if tm.enable_rowwise_temporal else "pointwise", B, T, V, H, W,
+                inner, heads, torch.empty(rows, inner, device=dev, dtype=dt), peer_kv=peer_kv,
+                kv_loc=kv_loc, kv_all=kv_all)
         for li, bp in enumerate(p["blocks"]):
             # --- spatial BasicTransformerBlock: self-attn, cross-attn to text, GEGLU FF
             n = bp["n1"]
@@ -553,7 +634,8 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                                        stride_outer=V * S, stride_inner=0)
                 tm.temporal_transformer_blocks[li].run(
                     p["tp"][li], h, tabs["t"], S, ws, attend,
-                    tm.time_mixer.batch_alpha(B, cd["dis_t"]["t"], dev), T * V * S)
+                    tm.time_mixer.batch_alpha(B, cd["dis_t"]["t"], dev), T * V * S,
+                    qkv_attend=tp_sharded)
         h16 = torch.empty(h.shape, device=dev, dtype=dt)
         _ops.act_cast(h, h16)
         return gemm(h16, p["proj_out"], epilogue=_lib.EPI_RESID, resid=x)
@@ -606,7 +688,9 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
 
     def _conditions(self, geo, H, W, encoder_hidden_states, condition_image_tensor,
                     added_time_ids, disable_crossview, disable_temporal, mask):
-        key = (geo, H, W) + tuple(self._tkey(t) for t in (
+        # the frame-index tables depend on where a frame shard sits in the window
+        shard = (self.shard.T, self.shard.t_offset) if self._frame_sharded() else None
+        key = (geo, H, W, shard) + tuple(self._tkey(t) for t in (
             encoder_hidden_states, condition_image_tensor, added_time_ids, disable_crossview,
             disable_temporal, mask))
         if key == self._cond_key:
@@ -672,6 +756,11 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         N, geo, dev = B * T * V, (B, T, V), sample.device
         if self._ws8_key != (B, T, V, H, W):     # one live E4M3 workspace
             self._ws8, self._ws8_key = {}, (B, T, V, H, W)
+        if self._frame_sharded():
+            if T != self.shard.T_loc:
+                raise ValueError("sample holds {} frames, the ShardPlan's shard {}".format(
+                    T, self.shard.T_loc))
+            self._peer_buffers(geo, H, W)
         cd = self._conditions(geo, H, W, encoder_hidden_states, condition_image_tensor,
                               added_time_ids, disable_crossview, disable_temporal,
                               crossview_attention_mask)

@@ -433,9 +433,10 @@ class CrossviewTemporalSD:
         and captures."""
         stateful = not self.is_dit and not hasattr(self.test_scheduler, "final_alpha_cumprod")
         # sharded steps contain NCCL / symmetric-memory exchanges: captured only on request
-        # (DWM_CUDA_GRAPH_SHARDED=1, not yet measured); multistep schedulers keep host state
-        sharded = self.sharding is not None and \
-            os.environ.get("DWM_CUDA_GRAPH_SHARDED", "0") != "1"
+        # (DWM_CUDA_GRAPH_SHARDED=1, not yet measured; DiT only, a sharded UNet step always
+        # runs eager); multistep schedulers keep host state
+        sharded = self.sharding is not None and (
+            not self.is_dit or os.environ.get("DWM_CUDA_GRAPH_SHARDED", "0") != "1")
         if self.sharding is not None and self.sharding.t_ways > 1 and \
                 len(getattr(self.model, "temporal_block_layers", ())) % 2 == 1:
             # the peer K,V buffers alternate per temporal block; a captured step with an odd
@@ -478,9 +479,15 @@ class CrossviewTemporalSD:
 
     def _denoise_step_unet(self, latents, conditions, timesteps, do_cfg):
         """CTSD-2.1 step: CFG batching, UNet forward, fused CFG + DDIM (eta 0) update
-        (reference ctsd.py:1536-1575 with the in-repo DDIMScheduler.step)."""
-        x = torch.cat([latents, latents]) if do_cfg else latents
-        t = torch.cat([timesteps, timesteps]) if do_cfg else timesteps
+        (reference ctsd.py:1536-1575 with the in-repo DDIMScheduler.step).  Under a ShardPlan
+        `latents` / `conditions` hold this rank's frames (and CFG branch, which the pair then
+        exchanges); the update runs on the local frames."""
+        plan = self.sharding
+        split_cfg = do_cfg and plan is not None and plan.cfg_ways == 2
+        self.model.shard = plan
+        both = do_cfg and not split_cfg
+        x = torch.cat([latents, latents]) if both else latents
+        t = torch.cat([timesteps, timesteps]) if both else timesteps
         out, _, _ = self.model(
             x.to(self.model_dtype), t,
             encoder_hidden_states=conditions["encoder_hidden_states"],
@@ -489,11 +496,16 @@ class CrossviewTemporalSD:
             disable_temporal=conditions.get("disable_temporal"),
             crossview_attention_mask=conditions.get("crossview_attention_mask"),
             added_time_ids=conditions.get("added_time_ids"))
+        pred = out[0].float().contiguous()
+        if split_cfg:   # [uncond ; cond] predictions of the local frames on both ranks
+            branch = pred
+            pred = torch.empty((2 * branch.shape[0],) + tuple(branch.shape[1:]),
+                               device=branch.device, dtype=branch.dtype)
+            plan.gather_cfg_tokens(branch, pred)
         sch = self.test_scheduler
         if not hasattr(sch, "final_alpha_cumprod"):
             # generic scheduler (e.g. DPM-Solver++ multistep, reference :1573-1575): CFG
             # combine, then the scheduler's own scalar-timestep step (it counts steps itself)
-            pred = out[0].float().contiguous()
             if do_cfg:
                 g = float(self.inference_config.get("guidance_scale", 1))
                 w = self.__dict__.get("_cfg_w")
@@ -507,7 +519,7 @@ class CrossviewTemporalSD:
             return latents
         sch.alphas_cumprod = sch.alphas_cumprod.to(latents.device)
         _ops.cfg_ddim_step(
-            out[0].float().contiguous(), latents,
+            pred, latents,
             timesteps.to(torch.int32).contiguous(), sch.alphas_cumprod,
             cfg=2 if do_cfg else 1,
             guidance_scale=self.inference_config.get("guidance_scale", 1),
@@ -575,7 +587,7 @@ class CrossviewTemporalSD:
         # end-to-end sharding (opendwm_b200.sharding.ShardPlan in self.sharding): every rank
         # builds the full noise / conditions (same generator seed), keeps its CFG branch and
         # frames for the steps, and the window is re-assembled before the decode
-        plan = self.sharding if self.is_dit else None
+        plan = self.sharding
         fs = slice(0, T)
         if plan is not None:
             fs = plan.frame_slice()

@@ -5,7 +5,8 @@
 
 Every rank builds the same seeded small DiT, runs diffusion-forcing denoise steps with the
 CFG x frame sharding plan, and the gathered latents are compared with an unsharded run of
-the same steps on rank 0.  Exit code 0 = match."""
+the same steps on rank 0.  Exit code 0 = match.  `--unet` checks the CTSD-2.1 UNet instead
+(`unet_main`)."""
 import os
 import sys
 
@@ -101,5 +102,50 @@ def main():
     sys.exit(0 if all_equal and worst == 0.0 else 1)
 
 
+def unet_main():
+    """--unet: every rank's sharded noise prediction of the CTSD-2.1 UNet (its CFG branch and
+    frames) against its own unsharded forward, relative to the output's range (GroupNorm
+    statistics are atomics, so within 2e-3 in 16 bit and 8e-2 in E4M3 rather than bit for bit).  Run it with and
+    without DWM_PEER_SCATTER=0 to check the symmetric-memory halo and K,V stores across GPUs."""
+    from test_unet_sharded_gpu import _forward, _forward_inputs, _model
+    from opendwm_b200.sharding import ShardPlan
+    from opendwm_b200 import lib
+    rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
+    torch.cuda.set_device(int(os.environ["LOCAL_RANK"]))
+    dev = torch.device("cuda")
+    dist.init_process_group("nccl", device_id=torch.device("cuda", torch.cuda.current_device()))
+    lib.set_option("attn_tc", 0)
+    t_ways = world // (2 if world >= 2 else 1)
+    cases = [(v, T, fp8) for v, T, fp8 in [("video", 8, False), ("video", 5, False),
+                                           ("pointwise", 11, False), ("video", 8, True)]
+             if T >= t_ways]
+    ok = True
+    for variant, T, fp8 in cases:
+        m = _model(variant, fp8)
+        x, t, c = _forward_inputs(T)
+        ref = _forward(m, x, t, c)
+        plan = ShardPlan(world, rank, T)
+        fs = plan.frame_slice()
+        half = slice(None) if plan.cfg_ways == 1 else slice(plan.cfg_rank, plan.cfg_rank + 1)
+        m.shard = plan
+        got = _forward(m, x[half, fs].contiguous(), t[half, fs].contiguous(),
+                       plan.local_conditions(c, cfg_doubled=True))
+        m.shard = None
+        err = torch.tensor([((got - ref[half, fs]).abs().max() / ref.abs().max()).item()],
+                           device=dev)
+        dist.all_reduce(err, op=dist.ReduceOp.MAX)
+        tol = 8e-2 if fp8 else 2e-3
+        ok = ok and err.item() <= tol
+        if rank == 0:
+            print("shard_check unet world=%d plan=%s T=%d shards=%s temporal=%s e4m3=%s "
+                  "peer_scatter=%s max_rel_err=%.3e (tolerance %.0e)" % (
+                      world, plan.parallelism, T, plan.counts, variant, fp8,
+                      plan.use_peer_scatter and plan.t_ways > 1, err.item(), tol), flush=True)
+        del m
+        torch.cuda.empty_cache()
+    dist.destroy_process_group()
+    sys.exit(0 if ok else 1)
+
+
 if __name__ == "__main__":
-    main()
+    unet_main() if "--unet" in sys.argv else main()
