@@ -48,6 +48,9 @@ int make_tmap_nd(CUtensorMap* map, const void* base, int rank, const uint64_t* d
 
 int sm_count();
 
+// true if p (which may be null) is a multiple of `bytes`, a power of two
+inline bool is_aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 #ifdef __CUDACC__
 // ---------------------------------------------------------------------------
 // device helpers

@@ -255,10 +255,9 @@ static int launch_ln_staged(const LnParams& p, cudaStream_t s) {
 template <typename T, bool DUAL>
 static int launch_ln2(const LnParams& p, cudaStream_t s) {
   const int need = (p.D / 4 + 31) / 32;
-  // staged path: no per-row residual input, rows 16-byte aligned, ring <= 220 KB, enough rows
-  const bool staged = g_ln_staged && !p.add_full && (p.ldx & 3) == 0 &&
-                      LNS_STAGES * LNS_ROWS * p.D * 4 <= 220 * 1024 && p.M >= 4096 &&
-                      (reinterpret_cast<uintptr_t>(p.x) & 15) == 0;
+  // staged path: no per-row residual input, ring <= 220 KB, enough rows (x and ldx are
+  // 16-byte aligned: dwm_b200_layernorm checks them)
+  const bool staged = g_ln_staged && !p.add_full && LNS_STAGES * LNS_ROWS * p.D * 4 <= 220 * 1024 && p.M >= 4096;
   if (staged) {
     if (need <= 3) return launch_ln_staged<T, 3, DUAL>(p, s);
     if (need <= 6) return launch_ln_staged<T, 6, DUAL>(p, s);
@@ -543,6 +542,7 @@ extern "C" int dwm_b200_lincomb2(const float* x, const float* y, const float* s0
 
 extern "C" int dwm_b200_axpy(const float* x, float* y, int64_t n, float a, dwm_stream_t stream) {
   DWM_REQUIRE(x && y && n > 0, "dwm_b200_axpy: bad arguments");
+  DWM_REQUIRE(is_aligned(x, 16) && is_aligned(y, 16), "dwm_b200_axpy: x and y must be 16-byte aligned");
   const unsigned grid = static_cast<unsigned>((n / 4 + 1 + 255) / 256);
   axpy_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, y, n, a);
   DWM_CHECK_CUDA(cudaGetLastError());
@@ -603,6 +603,20 @@ extern "C" int dwm_b200_layernorm(const dwm_layernorm_args* a, dwm_stream_t stre
   DWM_REQUIRE(a->ldx % 4 == 0 && a->ldo % 4 == 0, "dwm_b200_layernorm: ldx/ldo must be multiples of 4");
   if (a->shift || a->scale || a->shift2 || a->scale2)
     DWM_REQUIRE(a->mod_ld % 4 == 0, "dwm_b200_layernorm: mod_ld must be a multiple of 4");
+  // every fp32 operand is read (sum_out written) as float4
+  const float* f32s[] = {a->x, a->add_item, a->add_full, a->sum_out, a->weight, a->bias,
+                         a->shift, a->scale, a->shift2, a->scale2};
+  for (const float* q : f32s)
+    DWM_REQUIRE(is_aligned(q, 16),
+                "dwm_b200_layernorm: x, add_item, add_full, sum_out, weight, bias, shift, scale, shift2, scale2 "
+                "must be 16-byte aligned");
+  DWM_REQUIRE((!a->add_item || a->add_item_ld % 4 == 0) && (!a->add_full || a->add_full_ld % 4 == 0) &&
+                  (!a->sum_out || a->ld_sum % 4 == 0) && (!a->out2 || a->ldo2 % 4 == 0),
+              "dwm_b200_layernorm: add_item_ld, add_full_ld, ld_sum, ldo2 must be multiples of 4");
+  // four outputs per store: 8 bytes of 16-bit values, 4 bytes of E4M3
+  const uintptr_t out_align = a->dtype == DWM_E4M3 ? 4 : 8;
+  DWM_REQUIRE(is_aligned(a->out, out_align) && is_aligned(a->out2, out_align),
+              "dwm_b200_layernorm: out and out2 must be %d-byte aligned", (int)out_align);
   LnParams p;
   p.M = static_cast<int>(a->M); p.D = static_cast<int>(a->D);
   p.x = a->x; p.ldx = a->ldx;
@@ -620,7 +634,6 @@ extern "C" int dwm_b200_layernorm(const dwm_layernorm_args* a, dwm_stream_t stre
   if (a->dtype == DWM_E4M3) {
     DWM_REQUIRE(a->out_scale && (!a->out2 || a->out2_scale),
                 "dwm_b200_layernorm: E4M3 output needs out_scale (and out2_scale with out2)");
-    DWM_REQUIRE(!a->out2 || a->ldo2 % 4 == 0, "dwm_b200_layernorm: ldo2 must be a multiple of 4");
     return launch_ln<__nv_fp8_e4m3>(p, s);
   }
   set_last_error("dwm_b200_layernorm: dtype must be DWM_BF16, DWM_F16 or DWM_E4M3");
@@ -654,6 +667,10 @@ extern "C" int dwm_b200_quantize_rows(const void* x, int64_t M, int64_t K, int64
 
 extern "C" int dwm_b200_act_cast(const float* in, void* out, int64_t n, int act, int dtype, dwm_stream_t stream) {
   DWM_REQUIRE(in && out && n > 0, "dwm_b200_act_cast: bad arguments");
+  DWM_REQUIRE(act == DWM_ACT_NONE || act == DWM_ACT_SILU || act == DWM_ACT_GELU_TANH || act == DWM_ACT_GELU_ERF,
+              "dwm_b200_act_cast: activation %d is not implemented (NONE, SILU, GELU_TANH, GELU_ERF)", act);
+  DWM_REQUIRE(is_aligned(in, 16) && is_aligned(out, 8),
+              "dwm_b200_act_cast: in must be 16-byte and out 8-byte aligned");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const unsigned grid = static_cast<unsigned>((n / 4 + 1 + 255) / 256);
   if (dtype == DWM_BF16) act_cast_kernel<<<grid, 256, 0, s>>>(in, reinterpret_cast<__nv_bfloat16*>(out), n, act);

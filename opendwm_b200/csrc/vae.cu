@@ -11,16 +11,29 @@
 namespace dwm {
 
 // ---- GroupNorm statistics: sums[n][g] = (sum x, sum x^2) over (C/G channels, all pixels) ----
+// Every loaded float is widened to double before it is added or squared, and the per-thread
+// partials, the per-block shared-memory reduction and the cross-block atomics all stay in
+// double.  The apply kernel forms the variance as sum x^2 / n - mean^2, which cancels when
+// |mean| >> std: an fp32 accumulation lost every significant bit of the variance of groups
+// with |mean| / std ~ 1e3 and made it negative (NaN output) for constant groups.  The
+// kernels remain HBM-bound; the (sum, sum sq) format is what ShardPlan.reduce_group_sums
+// all-reduces across frame shards.
+__device__ __forceinline__ void gn_acc(double& s, double& q, float v) {
+  const double d = static_cast<double>(v);
+  s += d;
+  q = fma(d, d, q);
+}
+
 // block = 256 threads; thread handles float4 channel vector c4 = tid % (C/4) of pixels
 // tid / (C/4), +stride...  Partial sums are combined per group in shared memory, then one
 // double atomicAdd per (block, group).
 __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__ x, long long pixels, int C, int G,
                                                        long long pixels_per_block, double* __restrict__ sums) {
-  __shared__ float s_sum[64], s_sq[64];
+  __shared__ double s_sum[64], s_sq[64];
   const int n = blockIdx.y;
   const int vec = C >> 2;
   const int tid = threadIdx.x;
-  if (tid < 64) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
+  if (tid < 64) { s_sum[tid] = 0.0; s_sq[tid] = 0.0; }
   __syncthreads();
   const int c4 = tid % vec;
   const int prow = tid / vec;
@@ -28,13 +41,12 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
   const long long p0 = static_cast<long long>(blockIdx.x) * pixels_per_block;
   long long p1 = p0 + pixels_per_block;
   if (p1 > pixels) p1 = pixels;
-  float a = 0.f, b = 0.f;
+  double a = 0.0, b = 0.0;
   if (prow < rows_per_iter) {
     const float4* base = reinterpret_cast<const float4*>(x + static_cast<long long>(n) * pixels * C);
     for (long long p = p0 + prow; p < p1; p += rows_per_iter) {
       const float4 v = base[p * vec + c4];
-      a += v.x + v.y + v.z + v.w;
-      b += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+      gn_acc(a, b, v.x); gn_acc(a, b, v.y); gn_acc(a, b, v.z); gn_acc(a, b, v.w);
     }
   }
   const int g = (c4 * 4) / (C / G);
@@ -42,8 +54,8 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
   atomicAdd(&s_sq[g], b);
   __syncthreads();
   if (tid < G) {
-    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2], static_cast<double>(s_sum[tid]));
-    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2 + 1], static_cast<double>(s_sq[tid]));
+    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2], s_sum[tid]);
+    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2 + 1], s_sq[tid]);
   }
 }
 
@@ -53,42 +65,39 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
 // per thread and one double atomic per (block, group).
 __global__ void __launch_bounds__(1024) gn_stats_wide_kernel(const float* __restrict__ x, long long pixels, int C, int G,
                                                              long long pixels_per_block, double* __restrict__ sums) {
-  __shared__ float s_sum[64], s_sq[64];
+  __shared__ double s_sum[64], s_sq[64];
   const int n = blockIdx.y, tid = threadIdx.x;
   const int vec = C >> 2;
-  if (tid < 64) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
+  if (tid < 64) { s_sum[tid] = 0.0; s_sq[tid] = 0.0; }
   __syncthreads();
   const int c4 = tid % vec, prow = tid / vec, k = blockDim.x / vec;
   const long long p0 = static_cast<long long>(blockIdx.x) * pixels_per_block;
   long long p1 = p0 + pixels_per_block;
   if (p1 > pixels) p1 = pixels;
-  float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f, q0 = 0.f, q1 = 0.f, q2 = 0.f, q3 = 0.f;
+  double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0, q0 = 0.0, q1 = 0.0, q2 = 0.0, q3 = 0.0;
   const float4* base = reinterpret_cast<const float4*>(x + static_cast<long long>(n) * pixels * C);
   for (long long p = p0 + prow; p < p1; p += k) {
     const float4 v = base[p * vec + c4];
-    s0 += v.x; q0 += v.x * v.x;
-    s1 += v.y; q1 += v.y * v.y;
-    s2 += v.z; q2 += v.z * v.z;
-    s3 += v.w; q3 += v.w * v.w;
+    gn_acc(s0, q0, v.x); gn_acc(s1, q1, v.y); gn_acc(s2, q2, v.z); gn_acc(s3, q3, v.w);
   }
   const int cg = C / G;
-  const float ss[4] = {s0, s1, s2, s3}, qq[4] = {q0, q1, q2, q3};
+  const double ss[4] = {s0, s1, s2, s3}, qq[4] = {q0, q1, q2, q3};
   int cur = (c4 * 4) / cg;
-  float a = 0.f, b = 0.f;
+  double a = 0.0, b = 0.0;
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
     const int g = (c4 * 4 + e) / cg;
     if (g != cur) {
       atomicAdd(&s_sum[cur], a); atomicAdd(&s_sq[cur], b);
-      cur = g; a = 0.f; b = 0.f;
+      cur = g; a = 0.0; b = 0.0;
     }
     a += ss[e]; b += qq[e];
   }
   atomicAdd(&s_sum[cur], a); atomicAdd(&s_sq[cur], b);
   __syncthreads();
   if (tid < G) {
-    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2], static_cast<double>(s_sum[tid]));
-    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2 + 1], static_cast<double>(s_sq[tid]));
+    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2], s_sum[tid]);
+    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2 + 1], s_sq[tid]);
   }
 }
 
@@ -96,9 +105,9 @@ __global__ void __launch_bounds__(1024) gn_stats_wide_kernel(const float* __rest
 __global__ void __launch_bounds__(256) gn_stats_generic_kernel(const float* __restrict__ x, long long pixels, int C,
                                                                int G, long long pixels_per_block,
                                                                double* __restrict__ sums) {
-  __shared__ float s_sum[64], s_sq[64];
+  __shared__ double s_sum[64], s_sq[64];
   const int n = blockIdx.y, tid = threadIdx.x;
-  if (tid < 64) { s_sum[tid] = 0.f; s_sq[tid] = 0.f; }
+  if (tid < 64) { s_sum[tid] = 0.0; s_sq[tid] = 0.0; }
   __syncthreads();
   const int cg = C / G;
   const long long e0 = static_cast<long long>(blockIdx.x) * pixels_per_block * C;
@@ -107,21 +116,20 @@ __global__ void __launch_bounds__(256) gn_stats_generic_kernel(const float* __re
   const float* base = x + static_cast<long long>(n) * pixels * C;
   // consecutive threads read consecutive elements; accumulate runs of equal group locally
   int cur_g = -1;
-  float a = 0.f, b = 0.f;
+  double a = 0.0, b = 0.0;
   for (long long e = e0 + tid; e < e1; e += 256) {
     const int g = static_cast<int>(e % C) / cg;
     if (g != cur_g) {
       if (cur_g >= 0) { atomicAdd(&s_sum[cur_g], a); atomicAdd(&s_sq[cur_g], b); }
-      cur_g = g; a = 0.f; b = 0.f;
+      cur_g = g; a = 0.0; b = 0.0;
     }
-    const float v = base[e];
-    a += v; b += v * v;
+    gn_acc(a, b, base[e]);
   }
   if (cur_g >= 0) { atomicAdd(&s_sum[cur_g], a); atomicAdd(&s_sq[cur_g], b); }
   __syncthreads();
   if (tid < G) {
-    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2], static_cast<double>(s_sum[tid]));
-    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2 + 1], static_cast<double>(s_sq[tid]));
+    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2], s_sum[tid]);
+    atomicAdd(&sums[(static_cast<long long>(n) * G + tid) * 2 + 1], s_sq[tid]);
   }
 }
 
@@ -173,8 +181,9 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
     const double s = p.sums[(static_cast<long long>(n) * p.G + threadIdx.x) * 2];
     const double ss = p.sums[(static_cast<long long>(n) * p.G + threadIdx.x) * 2 + 1];
     const double mean_d = s / cnt;
-    s_stat[threadIdx.x] = make_float2(static_cast<float>(mean_d),
-                                      rsqrtf(static_cast<float>(ss / cnt - mean_d * mean_d) + p.eps));
+    // rounding of the sums can leave a (near-)constant group a variance slightly below 0
+    const double var_d = fmax(ss / cnt - mean_d * mean_d, 0.0);
+    s_stat[threadIdx.x] = make_float2(static_cast<float>(mean_d), rsqrtf(static_cast<float>(var_d) + p.eps));
   }
   if (MODE == SN_AMAX && threadIdx.x == 0) s_amax = 0u;
   if (p.zy && threadIdx.x < 64 && threadIdx.x < p.T) {
@@ -369,11 +378,25 @@ __global__ void __launch_bounds__(256) upsample_kernel(const float* __restrict__
 
 using namespace dwm;
 
+namespace {
+// float4 operands of the GroupNorm apply kernels; nullptr if all are aligned (null zy / zb too)
+const char* gn_align_check(const float* x, const double* sums, const float* gamma, const float* beta,
+                           const float* zy, const float* zb) {
+  if (!is_aligned(x, 16) || !is_aligned(gamma, 16) || !is_aligned(beta, 16) || !is_aligned(zy, 16) ||
+      !is_aligned(zb, 16))
+    return "x, gamma, beta (zy, zb) must be 16-byte aligned";
+  if (!is_aligned(sums, 8)) return "sums must be 8-byte aligned";
+  return nullptr;
+}
+}  // namespace
+
 extern "C" int dwm_b200_groupnorm_stats(const float* x, int64_t nb, int64_t pixels, int C, int groups,
                                         double* sums, dwm_stream_t stream) {
   DWM_REQUIRE(x && sums && nb > 0 && pixels > 0, "dwm_b200_groupnorm_stats: bad arguments");
   DWM_REQUIRE(C % 4 == 0 && groups > 0 && groups <= 64 && C % groups == 0,
               "dwm_b200_groupnorm_stats: need C %% 4 == 0, C %% groups == 0, groups <= 64 (got C=%d, groups=%d)", C, groups);
+  DWM_REQUIRE(is_aligned(x, 16) && is_aligned(sums, 8),
+              "dwm_b200_groupnorm_stats: x must be 16-byte and sums 8-byte aligned");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   DWM_CHECK_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * nb * groups, s));
   const int vec = C / 4;
@@ -412,6 +435,8 @@ extern "C" int dwm_b200_spatialnorm_silu(const float* x, int64_t nb, int64_t T, 
   DWM_REQUIRE(C % 4 == 0 && groups > 0 && C % groups == 0, "dwm_b200_spatialnorm_silu: bad C/groups");
   DWM_REQUIRE((zy == nullptr) == (zb == nullptr), "dwm_b200_spatialnorm_silu: zy and zb go together");
   DWM_REQUIRE(out_t0 >= 0 && out_t0 + T <= out_T, "dwm_b200_spatialnorm_silu: frame window outside out buffer");
+  DWM_REQUIRE(!gn_align_check(x, sums, gamma, beta, zy, zb) && is_aligned(out, 8),
+              "dwm_b200_spatialnorm_silu: x, gamma, beta, zy, zb must be 16-byte, sums and out 8-byte aligned");
   SnParams p;
   p.x = x; p.nb = (int)nb; p.T = (int)T; p.H = (int)H; p.W = (int)W; p.C = C; p.G = groups;
   p.sums = sums; p.eps = eps; p.gamma = gamma; p.beta = beta; p.zy = zy; p.zb = zb;
@@ -445,6 +470,8 @@ extern "C" int dwm_b200_groupnorm_silu_e4m3(const float* x, int64_t nb, int64_t 
               C, groups);
   DWM_REQUIRE(out_t0 >= 0 && out_t0 + T <= out_T, "dwm_b200_groupnorm_silu_e4m3: frame window outside out buffer");
   DWM_REQUIRE(nb <= 65535, "dwm_b200_groupnorm_silu_e4m3: nb <= 65535 required");
+  DWM_REQUIRE(!gn_align_check(x, sums, gamma, beta, nullptr, nullptr) && is_aligned(out, 4),
+              "dwm_b200_groupnorm_silu_e4m3: x, gamma, beta must be 16-byte, sums 8-byte, out 4-byte aligned");
   SnParams p;
   p.x = x; p.nb = (int)nb; p.T = (int)T; p.H = (int)H; p.W = (int)W; p.C = C; p.G = groups;
   p.sums = sums; p.eps = eps; p.gamma = gamma; p.beta = beta; p.zy = nullptr; p.zb = nullptr;
@@ -475,7 +502,7 @@ const char* gn_shard_check(const float* x, int64_t nb, int64_t T, int64_t H, int
   if (nb <= 0 || T <= 0 || H <= 0 || W <= 0 || nb > 65535) return "bad shape (need nb <= 65535)";
   if (C % c_align || groups <= 0 || groups > 64 || C % groups) return "bad C / groups";
   if (stat_frames < T) return "stat_frames < T";
-  return nullptr;
+  return gn_align_check(x, sums, gamma, beta, nullptr, nullptr);
 }
 
 SnParams gn_shard_params(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C, int groups,
@@ -499,9 +526,13 @@ void gn_launch_shape(const SnParams& p, int* threads, int* chunk, dim3* grid) {
   *grid = dim3(static_cast<unsigned>((per_img + *chunk - 1) / *chunk), static_cast<unsigned>(p.nb));
 }
 
-const char* gn_halo_check(void* out, void* prev_out, int64_t prev_out_T, void* next_out, int64_t next_out_T) {
+// `bytes`: the store width of four outputs (8 for 16-bit, 4 for E4M3)
+const char* gn_halo_check(void* out, void* prev_out, int64_t prev_out_T, void* next_out, int64_t next_out_T,
+                          uintptr_t bytes) {
   if (!out) return "null out";
   if ((prev_out && prev_out_T < 3) || (next_out && next_out_T < 3)) return "neighbour buffers hold >= 3 frames";
+  if (!is_aligned(out, bytes) || !is_aligned(prev_out, bytes) || !is_aligned(next_out, bytes))
+    return bytes == 8 ? "out, prev_out, next_out must be 8-byte aligned" : "out, prev_out, next_out must be 4-byte aligned";
   return nullptr;
 }
 
@@ -513,7 +544,7 @@ extern "C" int dwm_b200_groupnorm_silu_halo(const float* x, int64_t nb, int64_t 
                                             void* prev_out, int64_t prev_out_T, void* next_out,
                                             int64_t next_out_T, int dtype, dwm_stream_t stream) {
   const char* bad = gn_shard_check(x, nb, T, H, W, C, groups, sums, stat_frames, gamma, beta, 4);
-  if (!bad) bad = gn_halo_check(out, prev_out, prev_out_T, next_out, next_out_T);
+  if (!bad) bad = gn_halo_check(out, prev_out, prev_out_T, next_out, next_out_T, 8);
   DWM_REQUIRE(!bad, "dwm_b200_groupnorm_silu_halo: %s", bad);
   SnParams p = gn_shard_params(x, nb, T, H, W, C, groups, sums, stat_frames, eps, gamma, beta, apply_silu);
   p.out = out; p.prev_out = prev_out; p.prev_T = (int)prev_out_T; p.next_out = next_out; p.next_T = (int)next_out_T;
@@ -554,7 +585,7 @@ extern "C" int dwm_b200_groupnorm_silu_e4m3_halo(const float* x, int64_t nb, int
                                                  void* next_out, int64_t next_out_T, float* out_scale,
                                                  dwm_stream_t stream) {
   const char* bad = gn_shard_check(x, nb, T, H, W, C, groups, sums, stat_frames, gamma, beta, 16);
-  if (!bad) bad = gn_halo_check(out, prev_out, prev_out_T, next_out, next_out_T);
+  if (!bad) bad = gn_halo_check(out, prev_out, prev_out_T, next_out, next_out_T, 4);
   if (!bad && (!amax || !out_scale)) bad = "null amax / out_scale";
   DWM_REQUIRE(!bad, "dwm_b200_groupnorm_silu_e4m3_halo: %s", bad);
   SnParams p = gn_shard_params(x, nb, T, H, W, C, groups, sums, stat_frames, eps, gamma, beta, apply_silu);
@@ -573,6 +604,7 @@ extern "C" int dwm_b200_groupnorm_silu_e4m3_halo(const float* x, int64_t nb, int
 extern "C" int dwm_b200_upsample_nearest(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C,
                                          int compress_time, void* out, int dtype, dwm_stream_t stream) {
   DWM_REQUIRE(x && out && C % 4 == 0, "dwm_b200_upsample_nearest: bad arguments");
+  DWM_REQUIRE(is_aligned(x, 16) && is_aligned(out, 8), "dwm_b200_upsample_nearest: x must be 16-byte and out 8-byte aligned");
   int mode = 0;
   long long To = T;
   if (compress_time && T > 1) {

@@ -444,6 +444,9 @@ def euler_step_by_indices(model_output, sample, idx, sigmas, round_dtype=torch.f
     if idx.dtype != torch.int32:
         raise TypeError("idx must be int32")
     n = sample.numel()
+    if idx.numel() == 0 or n % idx.numel():
+        raise ValueError("sample has {} elements, not a multiple of idx's {}".format(
+            n, idx.numel()))
     inner = n // idx.numel()
     _l.check(_l.load().dwm_b200_euler_step_by_indices(
         model_output.data_ptr(), sample.data_ptr(), n, inner, idx.data_ptr(),
@@ -558,17 +561,37 @@ def groupnorm_stats(x, groups, sums=None):
     return sums
 
 
+def _check_gn_operands(sums, gamma, beta, nb, C, groups):
+    """GroupNorm statistics double [nb, groups, 2] and affine parameters fp32 [>= C]."""
+    if sums.dtype != torch.float64 or not sums.is_contiguous() or \
+            tuple(sums.shape) != (nb, groups, 2):
+        raise ValueError("sums must be contiguous float64 [{}, {}, 2]".format(nb, groups))
+    for t, name in ((gamma, "gamma"), (beta, "beta")):
+        _f32(t, name)
+        if t.numel() < C:
+            raise ValueError("{} has {} elements, the kernel reads {}".format(name, t.numel(), C))
+
+
 def spatialnorm_silu(x, sums, gamma, beta, out, *, groups, eps=1e-6, zy=None,
                      zb=None, out_t0=0, silu=True):
     """x fp32 [nb,T,H,W,C]; out 16-bit [nb,out_T,H,W,C]; zy/zb fp32 [nb,Tz,hz,wz,C]."""
     _f32(x, "x")
+    if x.dim() != 5 or not x.is_contiguous():
+        raise ValueError("x must be contiguous [nb, T, H, W, C]")
     nb, T, H, W, C = x.shape
-    if out.dim() != 5 or not out.is_contiguous() or out.shape[2:] != x.shape[2:]:
+    if out.dim() != 5 or not out.is_contiguous() or out.shape[0] != nb or out.shape[2:] != x.shape[2:]:
         raise ValueError("out must be contiguous [nb, out_T, H, W, C]")
+    _check_gn_operands(sums, gamma, beta, nb, C, groups)
     Tz = hz = wz = 0
+    if (zy is None) != (zb is None):
+        raise ValueError("zy and zb go together")
     if zy is not None:
-        _f32(zy, "zy")
-        _f32(zb, "zb")
+        for t, name in ((zy, "zy"), (zb, "zb")):
+            _f32(t, name)
+            if t.dim() != 5 or not t.is_contiguous() or t.shape[0] != nb or t.shape[4] != C:
+                raise ValueError("{} must be contiguous fp32 [nb, Tz, hz, wz, C]".format(name))
+        if zb.shape != zy.shape:
+            raise ValueError("zy and zb shapes differ")
         Tz, hz, wz = zy.shape[1:4]
     _l.check(_l.load().dwm_b200_spatialnorm_silu(
         x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), eps,
@@ -592,6 +615,7 @@ def groupnorm_silu_e4m3(x, sums, gamma, beta, out, scale, *, groups, eps=1e-6, o
     _f32(scale, "scale")
     if scale.numel() != nb or not scale.is_contiguous():
         raise ValueError("scale must be fp32 [nb]")
+    _check_gn_operands(sums, gamma, beta, nb, C, groups)
     _l.check(_l.load().dwm_b200_groupnorm_silu_e4m3(
         x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), eps,
         _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(), int(silu),
@@ -631,6 +655,7 @@ def groupnorm_silu_halo(x, sums, gamma, beta, out, *, groups, stat_frames, prev_
     neighbours' operands prev_out / next_out, a missing neighbour leaves a zero halo frame."""
     halo = _halo_args(x, out, prev_out, next_out, out.dtype)
     nb, T, H, W, C = x.shape
+    _check_gn_operands(sums, gamma, beta, nb, C, groups)
     _l.check(_l.load().dwm_b200_groupnorm_silu_halo(
         x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), stat_frames, eps,
         _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(), int(silu),
@@ -649,6 +674,7 @@ def groupnorm_silu_e4m3_amax(x, sums, gamma, beta, amax, *, groups, stat_frames,
     _f32(amax, "amax")
     if amax.numel() != nb or not amax.is_contiguous():
         raise ValueError("amax must be fp32 [nb]")
+    _check_gn_operands(sums, gamma, beta, nb, C, groups)
     _l.check(_l.load().dwm_b200_groupnorm_silu_e4m3_amax(
         x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), stat_frames, eps,
         _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(), int(silu),
@@ -663,6 +689,7 @@ def groupnorm_silu_e4m3_halo(x, sums, gamma, beta, amax, out, scale, *, groups, 
     gives for that amax), halo frames as in `groupnorm_silu_halo`."""
     halo = _halo_args(x, out, prev_out, next_out, FP8)
     nb, T, H, W, C = x.shape
+    _check_gn_operands(sums, gamma, beta, nb, C, groups)
     for t, name in ((amax, "amax"), (scale, "scale")):
         _f32(t, name)
         if t.numel() != nb or not t.is_contiguous():
@@ -677,6 +704,8 @@ def groupnorm_silu_e4m3_halo(x, sums, gamma, beta, amax, out, scale, *, groups, 
 
 def upsample_nearest(x, compress_time, dtype):
     _f32(x, "x")
+    if x.dim() != 5 or not x.is_contiguous():
+        raise ValueError("x must be contiguous [nb, T, H, W, C]")
     nb, T, H, W, C = x.shape
     To = T
     if compress_time and T > 1:
@@ -740,6 +769,9 @@ def lincomb2(x, y, s0, s1, out):
         if not t.is_contiguous():
             raise ValueError("lincomb2 needs contiguous tensors")
     n = x.numel()
+    if y.numel() != n or out.numel() != n or s1.numel() != s0.numel() or n % s0.numel():
+        raise ValueError("lincomb2: x {}, y {}, out {} must match and split into the {} items "
+                         "of s0 / s1 ({})".format(n, y.numel(), out.numel(), s0.numel(), s1.numel()))
     _l.check(_l.load().dwm_b200_lincomb2(
         x.data_ptr(), y.data_ptr(), s0.data_ptr(), s1.data_ptr(), n, n // s0.numel(),
         out.data_ptr(), _stream()), "dwm_b200_lincomb2")

@@ -180,6 +180,133 @@ def test_conv_argument_checks():
         pytest.fail("accepted or wrong message: %r" % failed)
 
 
+def _ln_args(**kw):
+    """A well-formed BF16 LayerNorm with every optional operand (resident kernel: M < 4096)."""
+    from opendwm_b200 import lib
+    a = lib.LayerNormArgs()
+    a.M, a.D, a.x, a.ldx = 64, 256, _addr(0), 260
+    a.add_item, a.add_item_ld, a.rows_per_item = _addr(1), 256, 16
+    a.add_full, a.add_full_ld = _addr(2), 264
+    a.sum_out, a.ld_sum = _addr(3), 256
+    a.weight, a.bias, a.eps = _addr(4), _addr(5), 1e-6
+    a.shift, a.scale, a.shift2, a.scale2, a.mod_ld = _addr(6), _addr(7), _addr(8), _addr(9), 1536
+    a.out, a.ldo, a.out2, a.ldo2, a.dtype = _addr(10), 256, _addr(11), 260, lib.DWM_BF16
+    for k, v in kw.items():
+        setattr(a, k, v)
+    return a
+
+
+def _ln_breaks():
+    from opendwm_b200 import lib
+    e4m3 = dict(dtype=lib.DWM_E4M3, out_scale=_addr(12), out2_scale=_addr(13))
+    out = [("%s+%d" % (f, m), {f: _addr(i, m)}, "16-byte aligned")
+           for i, (f, m) in enumerate((("x", 4), ("add_item", 8), ("add_full", 4), ("sum_out", 12),
+                                       ("weight", 4), ("bias", 8), ("shift", 4), ("scale", 8),
+                                       ("shift2", 12), ("scale2", 4)))]
+    out += [
+        ("add_item_ld 258", dict(add_item_ld=258), "multiples of 4"),
+        ("add_full_ld 262", dict(add_full_ld=262), "multiples of 4"),
+        ("ld_sum 257", dict(ld_sum=257), "multiples of 4"),
+        ("ldo2 258 bf16", dict(ldo2=258), "multiples of 4"),
+        ("ldo2 258 e4m3", dict(e4m3, ldo2=258), "multiples of 4"),
+        ("out+4 bf16", dict(out=_addr(10, 4)), "8-byte aligned"),
+        ("out2+2 bf16", dict(out2=_addr(11, 2)), "8-byte aligned"),
+        ("out+2 e4m3", dict(e4m3, out=_addr(10, 2)), "4-byte aligned"),
+    ]
+    return out
+
+
+def _fn(name, *args):
+    from opendwm_b200 import lib
+    rc = getattr(lib.load(), name)(*args)
+    return rc, lib.load().dwm_b200_last_error().decode()
+
+
+def _rowop_calls():
+    """(entry point, well-formed arguments, [(label, {argument index: value}, message)])."""
+    from opendwm_b200 import lib
+    A = _addr
+    gn = [A(0), 2, 3, 4, 6, 64, 16]   # x, nb, T, H, W, C, groups
+    ep = [A(2), A(3)]                 # gamma, beta
+    return [
+        ("dwm_b200_act_cast", [A(0), A(1), 1001, lib.ACT_SILU, lib.DWM_BF16, None], [
+            ("relu", {3: lib.ACT_RELU}, "not implemented"),
+            ("act 9", {3: 9}, "not implemented"),
+            ("in+8", {0: A(0, 8)}, "aligned"),
+            ("out+4", {1: A(1, 4)}, "aligned")]),
+        ("dwm_b200_axpy", [A(0), A(1), 1001, 0.5, None], [
+            ("x+4", {0: A(0, 4)}, "16-byte aligned"),
+            ("y+8", {1: A(1, 8)}, "16-byte aligned")]),
+        ("dwm_b200_upsample_nearest", [A(0), 2, 3, 4, 6, 64, 1, A(1), lib.DWM_BF16, None], [
+            ("x+8", {0: A(0, 8)}, "aligned"),
+            ("out+4", {7: A(1, 4)}, "aligned")]),
+        ("dwm_b200_groupnorm_stats", [A(0), 2, 72, 64, 16, A(1), None], [
+            ("x+4", {0: A(0, 4)}, "aligned"),
+            ("sums+4", {5: A(1, 4)}, "aligned")]),
+        ("dwm_b200_spatialnorm_silu",
+         gn + [A(1), 1e-6] + ep + [A(4), A(5), 2, 2, 3, 1, A(6), 5, 1, lib.DWM_BF16, None], [
+             ("x+4", {0: A(0, 4)}, "aligned"), ("sums+4", {7: A(1, 4)}, "aligned"),
+             ("gamma+8", {9: A(2, 8)}, "aligned"), ("beta+4", {10: A(3, 4)}, "aligned"),
+             ("zy+4", {11: A(4, 4)}, "aligned"), ("zb+12", {12: A(5, 12)}, "aligned"),
+             ("out+4", {17: A(6, 4)}, "aligned")]),
+        ("dwm_b200_groupnorm_silu_e4m3",
+         gn + [A(1), 1e-6] + ep + [1, A(6), 5, 1, A(7), None], [
+             ("x+4", {0: A(0, 4)}, "aligned"), ("gamma+4", {9: A(2, 4)}, "aligned"),
+             ("out+2", {12: A(6, 2)}, "aligned")]),
+        ("dwm_b200_groupnorm_silu_halo",
+         gn + [A(1), 6, 1e-6] + ep + [1, A(6), A(7), 5, A(8), 5, lib.DWM_BF16, None], [
+             ("x+4", {0: A(0, 4)}, "aligned"), ("beta+8", {11: A(3, 8)}, "aligned"),
+             ("out+4", {13: A(6, 4)}, "aligned"), ("prev_out+4", {14: A(7, 4)}, "aligned"),
+             ("next_out+2", {16: A(8, 2)}, "aligned")]),
+        ("dwm_b200_groupnorm_silu_e4m3_amax",
+         gn + [A(1), 6, 1e-6] + ep + [1, A(6), None], [
+             ("x+4", {0: A(0, 4)}, "aligned"), ("sums+4", {7: A(1, 4)}, "aligned")]),
+        ("dwm_b200_groupnorm_silu_e4m3_halo",
+         gn + [A(1), 6, 1e-6] + ep + [1, A(5), A(6), A(7), 5, A(8), 5, A(9), None], [
+             ("gamma+4", {10: A(2, 4)}, "aligned"), ("out+2", {14: A(6, 2)}, "aligned"),
+             ("next_out+1", {17: A(8, 1)}, "aligned")]),
+    ]
+
+
+def test_layernorm_argument_checks():
+    """dwm_b200_layernorm reads every fp32 operand as float4 and stores four outputs at a time:
+    it rejects each misaligned operand and pitch.  A misaligned x used to reach the resident
+    kernel as misaligned float4 loads."""
+    import pytest
+    _no_device()
+    rc, msg = _call("dwm_b200_layernorm", _ln_args())
+    assert rc < 0 and "cudaGetLastError" in msg, msg
+    failed = []
+    for name, kw, want in _ln_breaks():
+        rc, msg = _call("dwm_b200_layernorm", _ln_args(**kw))
+        if not (rc == -1 and re.search(want, msg)):
+            failed.append((name, rc, msg))
+    if failed:
+        pytest.fail("accepted or wrong message: %r" % failed)
+
+
+def test_rowop_and_groupnorm_argument_checks():
+    """act_cast, axpy, upsample_nearest and the GroupNorm entry points reject misaligned
+    operands (one broken argument per call), and act_cast an activation it does not implement
+    (ReLU used to return its input unchanged).  Each well-formed call passes every check and
+    fails only at its first CUDA call."""
+    import pytest
+    _no_device()
+    failed = []
+    for fn, args, breaks in _rowop_calls():
+        rc, msg = _fn(fn, *args)
+        assert rc == -2 and "failed:" in msg, (fn, msg)
+        for name, change, want in breaks:
+            bad = list(args)
+            for i, v in change.items():
+                bad[i] = v
+            rc, msg = _fn(fn, *bad)
+            if not (rc == -1 and re.search(want, msg)):
+                failed.append((fn, name, rc, msg))
+    if failed:
+        pytest.fail("accepted or wrong message: %r" % failed)
+
+
 def test_errors_without_gpu_are_loud():
     import pytest
     import torch

@@ -1,6 +1,15 @@
-"""Isolated timings of the non-GEMM kernels at north-star shapes."""
+"""Isolated timings of the non-GEMM kernels at north-star shapes.
+
+  python tools/kernel_bench.py                       all kernels
+  python tools/kernel_bench.py --only groupnorm_stats [--baseline-lib OTHER.so]
+
+--baseline-lib: a libdwm_b200.so built from another revision; its dwm_b200_groupnorm_stats is
+timed alternately with this tree's at the same shapes, and the two results compared."""
+import argparse
+import ctypes
 import json
 import os
+import subprocess
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -20,7 +29,69 @@ def timeit(fn, iters=10, warm=3):
     return e0.elapsed_time(e1) / iters
 
 
+# GroupNorm statistics shapes (nb, pixels, C): the four CTSD-2.1 UNet levels at 256 x 448 (12
+# volumes: 2 CFG branches x 6 views), and the 2-D VAE decoder's largest frame (6 views,
+# 256 x 448 pixels, 128 channels)
+GN_SHAPES = [(12, 32 * 56, 320), (12, 16 * 28, 640), (12, 8 * 14, 1280), (12, 4 * 7, 2560),
+             (6, 256 * 448, 128)]
+
+
+def _device_info():
+    """(card name, power limit) of GPU 0, read-only query."""
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        q = ""
+    return q or torch.cuda.get_device_name(0)
+
+
+def groupnorm_stats_bench(baseline_lib=None, rounds=5):
+    """ms per call of dwm_b200_groupnorm_stats (this tree, and `baseline_lib` alternately) and the
+    largest |difference| of the two results, per shape."""
+    from opendwm_b200 import lib
+    libs = {"this": lib.load()}
+    if baseline_lib:
+        other = ctypes.CDLL(baseline_lib)
+        other.dwm_b200_groupnorm_stats.restype = ctypes.c_int
+        other.dwm_b200_groupnorm_stats.argtypes = lib.SYMBOLS["dwm_b200_groupnorm_stats"][1]
+        libs["baseline"] = other
+    out = {"device": _device_info()}
+    for nb, pixels, C in GN_SHAPES:
+        x = torch.randn(nb, pixels, C, device="cuda") * 2 + 0.5
+        sums = {k: torch.empty(nb, 32, 2, device="cuda", dtype=torch.float64) for k in libs}
+
+        def call(h, s):
+            return lambda: lib.check(h.dwm_b200_groupnorm_stats(
+                x.data_ptr(), nb, pixels, C, 32, s.data_ptr(), torch.cuda.current_stream().cuda_stream),
+                "dwm_b200_groupnorm_stats")
+
+        fns = {k: call(libs[k], sums[k]) for k in libs}
+        times = {k: [] for k in libs}
+        for _ in range(rounds):                       # alternate the versions
+            for k, f in fns.items():
+                times[k].append(timeit(f, iters=50, warm=5))
+        r = {"gbs_this": x.numel() * 4 / min(times["this"]) / 1e6}
+        for k, t in times.items():
+            r["ms_" + k] = sorted(t)[len(t) // 2]
+            r["ms_%s_range" % k] = [min(t), max(t)]
+        if "baseline" in sums:
+            r["max_abs_diff"] = (sums["this"] - sums["baseline"]).abs().max().item()
+        out["%dx%dx%d" % (nb, pixels, C)] = r
+        print("groupnorm_stats", nb, pixels, C, r, flush=True)
+    return out
+
+
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--only", choices=["groupnorm_stats"])
+    ap.add_argument("--baseline-lib")
+    a = ap.parse_args()
+    if a.only == "groupnorm_stats":
+        res = groupnorm_stats_bench(a.baseline_lib)
+        os.makedirs("bench_out", exist_ok=True)
+        json.dump(res, open("bench_out/kernel_bench_groupnorm_stats.json", "w"), indent=1)
+        return
     res = {}
     D, heads, N, S, L = 1536, 24, 192, 448, 154
     dt = torch.bfloat16
@@ -101,6 +172,8 @@ def main():
     f = lambda: ops.layernorm(x, a16, weight=w, bias=b, add_item=emb, rows_per_item=S, sum_out=y)
     t = timeit(f)
     res["layernorm_affine_sum"] = dict(ms=t, gbs=(x.numel() * 8 + a16.numel() * 2) / t / 1e6)
+    del x, y, a16, qkv, qs, o, o2
+    res["groupnorm_stats"] = groupnorm_stats_bench(a.baseline_lib)
     for k, v in res.items():
         print(k, v, flush=True)
     os.makedirs("bench_out", exist_ok=True)
