@@ -33,6 +33,8 @@ and worst-case truncation are that loose for Hopper's accumulator on random data
 """
 import math
 import re
+import subprocess
+import sys
 
 import pytest
 import torch
@@ -143,8 +145,7 @@ class Epi:
         """float64 residual, gate, blend rows and alpha of each result row (None if absent).
         `bug` reads one of them from the wrong row (the self-test's wrong kernels)."""
         m = torch.arange(M)
-        dev = next(t.device for t in (self.resid, self.gate, self.blend_x) if t is not None) \
-            if self.kind == RESID else None
+        dev = next((t.device for t in (self.resid, self.gate, self.blend_x) if t is not None), None)
         item = m // self.rows_per_item if self.rows_per_item > 0 else torch.zeros_like(m)
         R = G = X = al = None
         if self.resid is not None:
@@ -173,12 +174,13 @@ def geglu_columns(N):
     return v, v + 128
 
 
-def epilogue_reference(z, P, K, e, out_dtype):
+def epilogue_reference(z, P, K, e, out_dtype, acc_err=None):
     """float64 (ref, tol) of the epilogue `e` applied to z = A W^T (float64, from the 16-bit
     operands the kernel reads), P = |A| |W|^T, [M, out_cols].  The kernel conforms where
     |out - ref| <= tol.
 
-    tol propagates the accumulation bound E = acc_bound(P, K) through the epilogue's fp32 steps
+    tol propagates the accumulation bound E = acc_bound(P, K) (or `acc_err`, a bound on
+    |acc - z| the caller derived otherwise, e.g. for FP8 operands) through the epilogue's fp32 steps
     (unit roundoff U32 = 2^-24 each, round to nearest):
       * pre = acc + bias: E_pre = E + U32 |pre|;
       * STORE / F32: L E_pre + the activation's own error (act_reference), with L its Lipschitz
@@ -199,7 +201,7 @@ def epilogue_reference(z, P, K, e, out_dtype):
     sub = 2.0 ** -25 if out_dtype == torch.float16 else 0.0
     b = e.bias.double()[:N].to(z.device) if e.bias is not None else torch.zeros(N, dtype=z.dtype, device=z.device)
     pre = z + b
-    e_pre = acc_bound(P, K) + U32 * pre.abs()
+    e_pre = (acc_bound(P, K) if acc_err is None else acc_err) + U32 * pre.abs()
     scale = P + b.abs()
     floor = 2.0 ** -20 * scale
     if e.kind in (STORE, F32):
@@ -285,7 +287,13 @@ def emulate(a, w, e, out_dtype, bug=None):
     b = e.bias.float().clone() if e.bias is not None else torch.zeros(N)
     if bug == "no bias on chunk 1":
         b[32:64] = 0
-    pre = acc + b
+    return emulate_epilogue(acc + b, e, out_dtype, bug)
+
+
+def emulate_epilogue(pre, e, out_dtype, bug=None):
+    """The fp32 epilogue after the bias, pre = acc + bias [M, N] fp32, then one rounding to the
+    output type."""
+    M, N = pre.shape
     if e.kind in (STORE, F32):
         y = _act32(pre, e.act)
     elif e.kind == RESID:
@@ -428,11 +436,11 @@ def _poison(n):
     return torch.tensor(POISON).repeat(n // 3 + 1)[:n]
 
 
-def poisoned_2d(t):
-    """CUDA view of t [R, C] inside an allocation with LD_PAD poisoned columns per row and
-    ROW_PAD poisoned rows after it."""
+def poisoned_2d(t, ld_pad=LD_PAD):
+    """CUDA view of t [R, C] inside an allocation with `ld_pad` poisoned columns per row and
+    ROW_PAD poisoned rows after it (E4M3: the NaN bytes 0x7F / 0xFF)."""
     R, C = t.shape
-    x = _poison((R + ROW_PAD) * (C + LD_PAD)).view(R + ROW_PAD, C + LD_PAD).to(t.dtype)
+    x = _poison((R + ROW_PAD) * (C + ld_pad)).view(R + ROW_PAD, C + ld_pad).to(t.dtype)
     x[:R, :C] = t
     return x.cuda()[:R, :C]
 
@@ -785,8 +793,9 @@ def test_conv_conforms(name, shape, label, dtype):
 # --------------------------------------------------------------------------------------------
 # which kernel ran
 # --------------------------------------------------------------------------------------------
-def _launched(fn):
-    """Template arguments of every gemm / conv wgmma kernel `fn` launches, in order."""
+def _launched(fn, types=False):
+    """Template arguments of every gemm / conv wgmma kernel `fn` launches, in order; with
+    `types`, each entry ends with the operand and 16-bit output type names (TA, T)."""
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         fn()
@@ -798,10 +807,23 @@ def _launched(fn):
             continue
         args = [re.sub(r"^\((int|bool)\)", "", s.strip()) for s in m.group(2).split(",")]
         if m.group(1) == "gemm":
-            found.append((int(args[3]), int(args[4])))
+            k = (int(args[3]), int(args[4]))
         else:
-            found.append((int(args[3]), int(args[4]), args[5] in ("true", "1")))
+            k = (int(args[3]), int(args[4]), args[5] in ("true", "1"))
+        found.append(k + tuple(a.split("::")[-1] for a in args[:2]) if types else k)
     return found
+
+
+def run_isolated(module, func):
+    """Runs module.func() (a check built on _launched) in a fresh Python process and fails with
+    its output if it fails.  The profiler loses kernels in a process with a history: on an H100
+    (torch 2.11, CUDA 12.8) a kernel launched in a profile went unrecorded once a CUDA graph had
+    been captured since the process's first profile, or, with CUPTI kept up between profiles,
+    once 20 s had passed.  A fresh process profiles only this check's own launches."""
+    code = "import sys; sys.path[:0] = %r; import %s as m; m.%s()" % (sys.path, module, func)
+    flags = ["-s"] if sys.flags.no_user_site else []
+    r = subprocess.run([sys.executable, *flags, "-c", code], capture_output=True, text=True, timeout=1200)
+    assert r.returncode == 0, "%s.%s failed:\n%s\n%s" % (module, func, r.stdout[-3000:], r.stderr[-6000:])
 
 
 def _selection_shapes(sms):
@@ -822,6 +844,11 @@ def _selection_shapes(sms):
 
 @pytest.mark.gpu
 def test_kernel_selection():
+    """check_kernel_selection, in a process of its own (run_isolated)."""
+    run_isolated("test_gemm_conformance_gpu", "check_kernel_selection")
+
+
+def check_kernel_selection():
     """The launched kernel's template arguments (NT, CL; CBN, CL, HALO) are the ones
     linear_kernel / conv_kernel predict, on both sides of each threshold, for every option
     setting the conformance cases use; and every kernel named in a case label is among them."""
