@@ -193,6 +193,17 @@ typedef struct dwm_attention_args {
   int seq_kv;
   int inner_kv;
   int64_t kv_stride_outer, kv_stride_inner;
+  /* Mask row of query unit 0 (>= 0; 0 = the unsharded meaning): query unit u = jq / inner reads
+   * mask row mask_q_offset + u, while key units index the mask over all n_outer units.  Used
+   * when the view axis is sharded: queries are the V_local views from v_offset, keys / values
+   * (kv) the gathered views of every rank, and mask_q_offset = v_offset.  With a mask and
+   * mask_q_offset > 0, mask_q_offset + (seq - 1) / inner must be < n_outer (the last query unit
+   * reads a mask row).  Separate K,V with a unit mask and whole
+   * units (seq_kv = n_outer * inner_kv, inner_kv = inner <= 128, n_outer <= 32, seq_kv > 64,
+   * unit strides 1) runs on the wgmma kernel that also runs the unsharded call over all units,
+   * and every local query row is bit-identical to its row of that call; separate K,V without a
+   * mask runs on the mma.sync kernel. */
+  int mask_q_offset;
 } dwm_attention_args;
 
 int dwm_b200_attention(const dwm_attention_args* args, dwm_stream_t stream);

@@ -48,6 +48,7 @@ struct AttnParams {
   const unsigned char* mask;  // [mask_batches, n_outer, n_outer] (1 = attend) or null
   int mask_div;               // mask batch = g0 / mask_div
   int n_outer;
+  int mask_q0;                // mask row of query unit 0 (the view offset of a view shard)
   float scale_log2;           // softmax scale * log2(e)
 };
 
@@ -168,8 +169,8 @@ __global__ void __launch_bounds__(NW * 32, NW == 4 ? 4 : 1) attn_kernel(const At
   const unsigned char* mrow1 = nullptr;
   if (p.mask) {
     const unsigned char* mb = p.mask + static_cast<long long>(g0 / p.mask_div) * p.n_outer * p.n_outer;
-    mrow0 = mb + (jq0 < p.seq ? jq0 / p.inner : 0) * p.n_outer;
-    mrow1 = mb + (jq1 < p.seq ? jq1 / p.inner : 0) * p.n_outer;
+    mrow0 = mb + (p.mask_q0 + (jq0 < p.seq ? jq0 / p.inner : 0)) * p.n_outer;
+    mrow1 = mb + (p.mask_q0 + (jq1 < p.seq ? jq1 / p.inner : 0)) * p.n_outer;
   }
 
   uint32_t qf[4][4];
@@ -336,11 +337,13 @@ static int launch_attn(const AttnParams& p, cudaStream_t s) {
 }
 
 // attention_wgmma.cu: contiguous sequences and gathered unit sequences (cross-view /
-// temporal row-wise, optional unit mask)
+// temporal row-wise, optional unit mask; local query views against separate gathered K,V)
 bool attn_tc_eligible(const dwm_attention_args* a);
 bool attn_tcg_eligible(const dwm_attention_args* a);
+bool attn_tcg_kv_eligible(const dwm_attention_args* a);
 int attn_wgmma_launch(const dwm_attention_args* a, cudaStream_t s);
 int attn_tcg_launch(const dwm_attention_args* a, cudaStream_t s);
+int attn_tcg_kv_launch(const dwm_attention_args* a, cudaStream_t s);
 
 }  // namespace dwm
 
@@ -359,6 +362,15 @@ extern "C" int dwm_b200_attention(const dwm_attention_args* a, dwm_stream_t stre
   if (a->split > 0)
     DWM_REQUIRE(a->out2 && a->ldo2 % 8 == 0 && a->split < a->seq, "dwm_b200_attention: bad split/out2");
   if (a->mask) DWM_REQUIRE(a->mask_div > 0 && a->n_outer > 0, "dwm_b200_attention: mask needs mask_div, n_outer");
+  DWM_REQUIRE(a->mask_q_offset >= 0, "dwm_b200_attention: mask_q_offset must be >= 0, got %d", a->mask_q_offset);
+  if (a->mask && a->mask_q_offset > 0)
+    DWM_REQUIRE(static_cast<long long>(a->mask_q_offset) + (a->seq - 1) / a->inner < a->n_outer,
+                "dwm_b200_attention: query units [%d, %d) lie outside the %d mask rows", a->mask_q_offset,
+                a->mask_q_offset + (a->seq - 1) / a->inner + 1, a->n_outer);
+  if (a->kv)
+    DWM_REQUIRE(a->ld_kv % 8 == 0 && a->k_col % 8 == 0 && a->v_col % 8 == 0 && a->seq_kv > 0 && a->inner_kv > 0 &&
+                    (reinterpret_cast<uintptr_t>(a->kv) & 15) == 0,
+                "dwm_b200_attention: bad separate kv description");
   {
     // contiguous sequences (joint / dual attention) and gathered unit sequences (cross-view /
     // temporal row-wise) run on the wgmma kernel; the rest (pointwise temporal, separate K,V,
@@ -369,12 +381,9 @@ extern "C" int dwm_b200_attention(const dwm_attention_args* a, dwm_stream_t stre
     }
     if (g_attn_tc >= 1 && attn_tc_eligible(a)) return attn_wgmma_launch(a, reinterpret_cast<cudaStream_t>(stream));
     if (g_attn_tc >= 1 && attn_tcg_eligible(a)) return attn_tcg_launch(a, reinterpret_cast<cudaStream_t>(stream));
+    if (g_attn_tc >= 1 && attn_tcg_kv_eligible(a)) return attn_tcg_kv_launch(a, reinterpret_cast<cudaStream_t>(stream));
   }
   const long long groups = static_cast<long long>(a->group_dims[0]) * a->group_dims[1] * a->group_dims[2];
-  if (a->kv)
-    DWM_REQUIRE(a->ld_kv % 8 == 0 && a->k_col % 8 == 0 && a->v_col % 8 == 0 && a->seq_kv > 0 && a->inner_kv > 0 &&
-                    (reinterpret_cast<uintptr_t>(a->kv) & 15) == 0,
-                "dwm_b200_attention: bad separate kv description");
   const int seq_max = (a->kv && a->seq_kv > a->seq) ? a->seq_kv : a->seq;
   const long long q_tiles = seq_max <= 32 ? 1 : (a->seq + 63) / 64;
   DWM_REQUIRE(groups * a->heads * q_tiles < (1ll << 31), "dwm_b200_attention: grid too large");
@@ -396,7 +405,7 @@ extern "C" int dwm_b200_attention(const dwm_attention_args* a, dwm_stream_t stre
   p.ogs0 = a->out_group_strides[0]; p.ogs1 = a->out_group_strides[1]; p.ogs2 = a->out_group_strides[2];
   p.oso = a->out_stride_outer; p.osi = a->out_stride_inner;
   p.split = a->split; p.out2 = a->out2; p.ldo2 = a->ldo2;
-  p.mask = a->mask; p.mask_div = a->mask_div; p.n_outer = a->n_outer;
+  p.mask = a->mask; p.mask_div = a->mask_div; p.n_outer = a->n_outer; p.mask_q0 = a->mask_q_offset;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (a->dtype == DWM_BF16) return launch_attn<__nv_bfloat16>(p, s);

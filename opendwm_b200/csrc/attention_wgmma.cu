@@ -17,6 +17,13 @@
 // units (upt * inner <= 128 rows) straight from the un-permuted q|k|v buffer — the
 // reference's two 264 MB permutes and its [512,168,168] mask never exist.  The view mask is
 // a per-row bit set over key units, expanded once per key block to a 128-bit column mask.
+//
+// Separate K,V (template flag SKV, gathered sequences only): queries are the local views of a
+// view shard, keys / values the gathered views of every rank in a second buffer with its own
+// 5-D tensor map.  Key blocks, their unit count `upt` and the mask columns are those of the
+// unsharded launch, and query unit u reads mask row mask_q0 + u, so each local query row sees
+// the same key blocks in the same order with the same arithmetic as its row of the unsharded
+// launch: its output is bit-identical.
 #include <string.h>
 
 #include "common.cuh"
@@ -46,6 +53,9 @@ struct FaParams {
   int inner, n_out, upt, g1n;
   long long out_gs1, out_so;
   const unsigned char* mask; int mask_div, mask_n;
+  // key / value columns of head 0 (in the qkv map, or in the K,V map with SKV), key units
+  // (n_out without SKV) and the mask row of query unit 0
+  int kcol, vcol, n_out_k, mask_q0;
 };
 
 // Descriptor of an MN-major operand (V: keys x head_dim, head_dim contiguous) written by TMA
@@ -66,10 +76,13 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-template <typename T, bool G>
+template <typename T, bool G, bool SKV>
 __global__ void __launch_bounds__(fa::THREADS, 1)
-    attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap, const FaParams p) {
+    attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_kv,
+                      const FaParams p) {
   using namespace fa;
+  static_assert(G || !SKV, "separate K,V needs gathered sequences");
+  const CUtensorMap* kvmap = SKV ? &tmap_kv : &tmap;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sq = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // Q  [16 KB]
   uint8_t* skv = sq + TILE;                                                     // [stages][K | V]
@@ -91,6 +104,7 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
   }
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap);
+    if constexpr (SKV) tma_prefetch_desc(&tmap_kv);
     mbar_init(q_full, 1);
     mbar_init(q_empty, CONSUMER_WARPS);
     for (int i = 0; i < KV_STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], CONSUMER_WARPS); }
@@ -125,15 +139,15 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
             const int g02 = g2 / p.g1n, i12 = g2 - g02 * p.g1n;
             tma_prefetch_5d(&tmap, h2 * HD, 0, qt2 * p.upt, i12, g02);
             for (int kb = 0; kb < p.n_kb; ++kb) {
-              tma_prefetch_5d(&tmap, p.D + h2 * HD, 0, kb * p.upt, i12, g02);
-              tma_prefetch_5d(&tmap, 2 * p.D + h2 * HD, 0, kb * p.upt, i12, g02);
+              tma_prefetch_5d(kvmap, p.kcol + h2 * HD, 0, kb * p.upt, i12, g02);
+              tma_prefetch_5d(kvmap, p.vcol + h2 * HD, 0, kb * p.upt, i12, g02);
             }
           } else {
             const int r2 = static_cast<int>(g2 * p.group_stride);
             tma_prefetch_2d(&tmap, h2 * HD, r2 + qt2 * BQ);
             for (int kb = 0; kb < p.n_kb; ++kb) {
-              tma_prefetch_2d(&tmap, p.D + h2 * HD, r2 + kb * BK);
-              tma_prefetch_2d(&tmap, 2 * p.D + h2 * HD, r2 + kb * BK);
+              tma_prefetch_2d(&tmap, p.kcol + h2 * HD, r2 + kb * BK);
+              tma_prefetch_2d(&tmap, p.vcol + h2 * HD, r2 + kb * BK);
             }
           }
         }
@@ -146,11 +160,11 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
           mbar_expect_tx(&kv_full[kvs], 2 * tile_tx);
           uint8_t* st = skv + kvs * 2 * TILE;
           if constexpr (G) {
-            tma_load_5d(&tmap, &kv_full[kvs], st, p.D + h * HD, 0, kb * p.upt, i1, g0, kEvictLast);
-            tma_load_5d(&tmap, &kv_full[kvs], st + TILE, 2 * p.D + h * HD, 0, kb * p.upt, i1, g0, kEvictLast);
+            tma_load_5d(kvmap, &kv_full[kvs], st, p.kcol + h * HD, 0, kb * p.upt, i1, g0, kEvictLast);
+            tma_load_5d(kvmap, &kv_full[kvs], st + TILE, p.vcol + h * HD, 0, kb * p.upt, i1, g0, kEvictLast);
           } else {
-            tma_load_2d(&tmap, &kv_full[kvs], st, p.D + h * HD, row0 + kb * BK, kEvictLast);
-            tma_load_2d(&tmap, &kv_full[kvs], st + TILE, 2 * p.D + h * HD, row0 + kb * BK, kEvictLast);
+            tma_load_2d(&tmap, &kv_full[kvs], st, p.kcol + h * HD, row0 + kb * BK, kEvictLast);
+            tma_load_2d(&tmap, &kv_full[kvs], st + TILE, p.vcol + h * HD, row0 + kb * BK, kEvictLast);
           }
           if (++kvs == KV_STAGES) { kvs = 0; kvph ^= 1; }
         }
@@ -183,9 +197,10 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
           row_ok[hi] = u < p.upt && qo[hi] < p.n_out;
           if (p.mask && row_ok[hi]) {
             const int g0 = g / p.g1n;
-            const unsigned char* mr = p.mask + (static_cast<long long>(g0 / p.mask_div) * p.mask_n + qo[hi]) * p.mask_n;
+            const unsigned char* mr =
+                p.mask + (static_cast<long long>(g0 / p.mask_div) * p.mask_n + p.mask_q0 + qo[hi]) * p.mask_n;
             uint32_t al = 0u;
-            for (int ko = 0; ko < p.n_out; ++ko) al |= (__ldg(mr + ko) != 0 ? 1u : 0u) << ko;
+            for (int ko = 0; ko < p.n_out_k; ++ko) al |= (__ldg(mr + ko) != 0 ? 1u : 0u) << ko;
             allowed[hi] = al;
           }
         }
@@ -207,7 +222,7 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
             unsigned __int128 cm = 0;
             for (int u2 = 0; u2 < p.upt; ++u2) {
               const int ko = kb * p.upt + u2;
-              if (ko < p.n_out && ((allowed[hi] >> ko) & 1u)) cm |= ones << (u2 * p.inner);
+              if (ko < p.n_out_k && ((allowed[hi] >> ko) & 1u)) cm |= ones << (u2 * p.inner);
             }
             cmw[hi][0] = static_cast<uint32_t>(cm);
             cmw[hi][1] = static_cast<uint32_t>(cm >> 32);
@@ -319,13 +334,15 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
   }
 }
 
-template <typename T, bool G>
+template <typename T, bool G, bool SKV>
 static int launch_attn_wgmma(const dwm_attention_args* a, cudaStream_t s) {
   using namespace fa;
   FaParams p;
   memset(&p, 0, sizeof(p));
-  CUtensorMap tm;
+  CUtensorMap tm, tm_kv;
   long long groups;
+  p.kcol = static_cast<int>(SKV ? a->k_col : a->D);
+  p.vcol = static_cast<int>(SKV ? a->v_col : 2 * a->D);
   if (G) {
     // merge the (optional) third group dim into the second: row offset i1*gs1 + i2*gs2 with
     // gs1 == gd2*gs2 is (i1*gd2 + i2)*gs2 (checked by attn_tcg_eligible)
@@ -334,25 +351,40 @@ static int launch_attn_wgmma(const dwm_attention_args* a, cudaStream_t s) {
     const long long ogs1 = a->group_dims[2] > 1 ? a->out_group_strides[2] : a->out_group_strides[1];
     p.inner = a->inner;
     p.n_out = a->seq / a->inner;
+    p.n_out_k = SKV ? a->seq_kv / a->inner_kv : p.n_out;
+    // key blocks of `upt` units, as many as the unsharded launch over all n_out_k units takes
     p.upt = 128 / a->inner;
-    if (p.upt > p.n_out) p.upt = p.n_out;
+    if (p.upt > p.n_out_k) p.upt = p.n_out_k;
     p.g1n = static_cast<int>(gd1);
     p.out_gs1 = ogs1;
     p.out_so = a->out_stride_outer;
-    p.mask = a->mask; p.mask_div = a->mask_div; p.mask_n = a->n_outer;
+    p.mask = a->mask; p.mask_div = a->mask_div; p.mask_n = a->n_outer; p.mask_q0 = a->mask_q_offset;
     groups = a->group_dims[0] * gd1;
     const uint64_t eb = 2;
-    const uint64_t dims[5] = {static_cast<uint64_t>(3 * a->D), static_cast<uint64_t>(a->inner),
+    const uint32_t box[5] = {64u, static_cast<uint32_t>(a->inner), static_cast<uint32_t>(p.upt), 1u, 1u};
+    if (SKV) {
+      const long long kgs1 = a->group_dims[2] > 1 ? a->kv_group_strides[2] : a->kv_group_strides[1];
+      const long long kcols = (a->k_col > a->v_col ? a->k_col : a->v_col) + a->D;
+      const uint64_t kdims[5] = {static_cast<uint64_t>(kcols), static_cast<uint64_t>(a->inner_kv),
+                                 static_cast<uint64_t>(p.n_out_k), static_cast<uint64_t>(gd1),
+                                 static_cast<uint64_t>(a->group_dims[0])};
+      const uint64_t kst[4] = {static_cast<uint64_t>(a->ld_kv) * eb,
+                               static_cast<uint64_t>(a->kv_stride_outer * a->ld_kv) * eb,
+                               static_cast<uint64_t>(kgs1 * a->ld_kv) * eb,
+                               static_cast<uint64_t>(a->kv_group_strides[0] * a->ld_kv) * eb};
+      int rc = make_tmap_nd(&tm_kv, a->kv, 5, kdims, kst, box, 2);
+      if (rc) return rc;
+    }
+    const uint64_t dims[5] = {static_cast<uint64_t>(SKV ? a->D : 3 * a->D), static_cast<uint64_t>(a->inner),
                               static_cast<uint64_t>(p.n_out), static_cast<uint64_t>(gd1),
                               static_cast<uint64_t>(a->group_dims[0])};
     const uint64_t st[4] = {static_cast<uint64_t>(a->ld) * eb, static_cast<uint64_t>(a->stride_outer * a->ld) * eb,
                             static_cast<uint64_t>(gs1 * a->ld) * eb,
                             static_cast<uint64_t>(a->group_strides[0] * a->ld) * eb};
-    const uint32_t box[5] = {64u, static_cast<uint32_t>(a->inner), static_cast<uint32_t>(p.upt), 1u, 1u};
     int rc = make_tmap_nd(&tm, a->qkv, 5, dims, st, box, 2);
     if (rc) return rc;
     p.q_tiles = (p.n_out + p.upt - 1) / p.upt;
-    p.n_kb = p.q_tiles;
+    p.n_kb = (p.n_out_k + p.upt - 1) / p.upt;
   } else {
     groups = a->group_dims[0];
     const long long rows_total = groups * a->group_strides[0];
@@ -369,7 +401,8 @@ static int launch_attn_wgmma(const dwm_attention_args* a, cudaStream_t s) {
   p.out = a->out; p.ldo = a->ldo; p.out_group_stride = a->out_group_strides[0];
   p.split = a->split; p.out2 = a->out2; p.ldo2 = a->ldo2;
   p.scale_log2 = a->scale * 1.4426950408889634f;
-  auto kern = attn_wgmma_kernel<T, G>;
+  if (!SKV) tm_kv = tm;
+  auto kern = attn_wgmma_kernel<T, G, SKV>;
   static bool attr_set = false;
   if (!attr_set) {
     DWM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
@@ -378,7 +411,7 @@ static int launch_attn_wgmma(const dwm_attention_args* a, cudaStream_t s) {
   const long long items = groups * a->heads * p.q_tiles;
   const long long slots = sm_count();
   const int grid = static_cast<int>(items < slots ? items : slots);
-  kern<<<grid, THREADS, SMEM_BYTES, s>>>(tm, p);
+  kern<<<grid, THREADS, SMEM_BYTES, s>>>(tm, tm_kv, p);
   DWM_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -412,16 +445,48 @@ bool attn_tcg_eligible(const dwm_attention_args* a) {
   return groups * a->heads * 8 < (1ll << 31);
 }
 
+// local query units of a view shard against the gathered units of every view in a separate K,V
+// buffer, with the [B, n_outer, n_outer] unit mask (cross-view row-wise attention under a view
+// plan).  The key side must be a sequence the unsharded launch runs here (attn_tcg_eligible with
+// the key geometry), so the key blocks are the same.  Separate K,V without a mask (frame-sharded
+// temporal attention, text cross-attention) stays on the mma.sync kernel.
+bool attn_tcg_kv_eligible(const dwm_attention_args* a) {
+  if (a->kv == nullptr || a->mask == nullptr || a->split > 0) return false;
+  if (a->inner <= 0 || a->inner > 128 || a->inner_kv != a->inner || a->seq_kv <= 64) return false;
+  if (a->seq % a->inner || a->seq_kv % a->inner_kv || a->stride_inner != 1 || a->out_stride_inner != 1 ||
+      a->kv_stride_inner != 1)
+    return false;
+  const long long n_out_k = a->seq_kv / a->inner_kv;
+  if (n_out_k > 32 || a->n_outer != n_out_k) return false;
+  if (a->k_col + a->D > a->ld_kv || a->v_col + a->D > a->ld_kv || a->D > a->ld) return false;
+  if (a->group_dims[2] > 1 &&
+      (a->group_strides[1] != a->group_dims[2] * a->group_strides[2] ||
+       a->out_group_strides[1] != a->group_dims[2] * a->out_group_strides[2] ||
+       a->kv_group_strides[1] != a->group_dims[2] * a->kv_group_strides[2]))
+    return false;
+  if (a->stride_outer <= 0 || a->group_strides[0] <= 0 || a->kv_stride_outer <= 0 || a->kv_group_strides[0] <= 0)
+    return false;
+  const long long groups = a->group_dims[0] * a->group_dims[1] * a->group_dims[2];
+  return groups * a->heads * 8 < (1ll << 31);
+}
+
 int attn_wgmma_launch(const dwm_attention_args* a, cudaStream_t s) {
-  if (a->dtype == DWM_BF16) return launch_attn_wgmma<__nv_bfloat16, false>(a, s);
-  if (a->dtype == DWM_F16) return launch_attn_wgmma<__half, false>(a, s);
+  if (a->dtype == DWM_BF16) return launch_attn_wgmma<__nv_bfloat16, false, false>(a, s);
+  if (a->dtype == DWM_F16) return launch_attn_wgmma<__half, false, false>(a, s);
   set_last_error("dwm_b200_attention: dtype must be DWM_BF16 or DWM_F16, got %d", a->dtype);
   return -1;
 }
 
 int attn_tcg_launch(const dwm_attention_args* a, cudaStream_t s) {
-  if (a->dtype == DWM_BF16) return launch_attn_wgmma<__nv_bfloat16, true>(a, s);
-  if (a->dtype == DWM_F16) return launch_attn_wgmma<__half, true>(a, s);
+  if (a->dtype == DWM_BF16) return launch_attn_wgmma<__nv_bfloat16, true, false>(a, s);
+  if (a->dtype == DWM_F16) return launch_attn_wgmma<__half, true, false>(a, s);
+  set_last_error("dwm_b200_attention: dtype must be DWM_BF16 or DWM_F16, got %d", a->dtype);
+  return -1;
+}
+
+int attn_tcg_kv_launch(const dwm_attention_args* a, cudaStream_t s) {
+  if (a->dtype == DWM_BF16) return launch_attn_wgmma<__nv_bfloat16, true, true>(a, s);
+  if (a->dtype == DWM_F16) return launch_attn_wgmma<__half, true, true>(a, s);
   set_last_error("dwm_b200_attention: dtype must be DWM_BF16 or DWM_F16, got %d", a->dtype);
   return -1;
 }

@@ -57,6 +57,7 @@ class AttentionArgs(ctypes.Structure):
         ("kv_group_strides", _i64 * 3),
         ("seq_kv", ctypes.c_int), ("inner_kv", ctypes.c_int),
         ("kv_stride_outer", _i64), ("kv_stride_inner", _i64),
+        ("mask_q_offset", ctypes.c_int),
     ]
 
 

@@ -278,7 +278,7 @@ def attention(qkv, out, *, D, heads, group_dims, group_strides, seq, inner=None,
               out_stride_outer=None, out_stride_inner=None, split=0, out2=None,
               mask=None, mask_div=1, scale=None, kv=None, k_col=0, v_col=0,
               kv_group_strides=None, seq_kv=None, inner_kv=None,
-              kv_stride_outer=0, kv_stride_inner=1):
+              kv_stride_outer=0, kv_stride_inner=1, mask_q_offset=0):
     """Gathered multi-head attention over the fused q|k|v buffer (or a separate
     key/value buffer `kv`); see dwm_attention_args in include/dwm_b200.h."""
     _rows2d(qkv, "qkv")
@@ -310,6 +310,7 @@ def attention(qkv, out, *, D, heads, group_dims, group_strides, seq, inner=None,
         if mask.dtype != torch.uint8 or mask.dim() != 3 or not mask.is_contiguous():
             raise TypeError("mask must be a contiguous uint8 [B, n, n] tensor")
         a.mask, a.mask_div, a.n_outer = mask.data_ptr(), mask_div, mask.shape[-1]
+    a.mask_q_offset = mask_q_offset
     a.scale = (D // heads) ** -0.5 if scale is None else scale
     if kv is not None:
         _rows2d(kv, "kv")

@@ -112,6 +112,44 @@ class AlphaBlender(torch.nn.Module):
             if a.numel() == 1 else a.flatten().contiguous()
 
 
+def _sharded_qkv_attend(D, eps, rows_full, remap, q_loc, attend, gather, peer_kv, kv_loc,
+                        kv_all):
+    """qkv_attend of a sharded block: K,V of the local rows are projected (+RMSNorm) straight
+    into the gathered buffer [rows_full, 2D], which keeps the UNSHARDED row layout on every
+    rank — through the GEMM epilogue's item row mapping `remap` into local AND peer memory
+    (fused scatter over NVLink, `peer_kv` a PeerKV of the exchanging group; one group barrier
+    per block), or into kv_loc followed by `gather(kv_loc, kv_all)` (an async all-gather) —
+    while the Q projection runs into q_loc; then `attend(kv_full, out)`."""
+
+    def project(p, a, w, nw, out, peer_out=None, **kw):
+        if p["qk_norm"]:
+            gemm(a, w, epilogue=_lib.EPI_QKNORM, out=out,
+                 q_norm_weight=nw, qk_region=D, qk_norm_regions=1,
+                 eps=eps, peer_out=peer_out, **kw)
+        else:
+            gemm(a, w, out=out, peer_out=peer_out, **kw)
+
+    def qkv_attend(p, a, out):
+        q, kv = p["qkv"].rows(0, D), p["qkv"].rows(D, 3 * D)
+        if peer_kv is not None:
+            # fused: the K,V GEMM epilogue scatters its tiles into every peer's
+            # gathered buffer over NVLink; one group barrier publishes them
+            kv_full, peers, hdl = peer_kv.next()
+            # the leading rows at this block's width (peers address their buffers the same way)
+            kv_full = kv_full.view(-1)[:rows_full * 2 * D].view(rows_full, 2 * D)
+            project(p, a, kv, p.get("nk"), kv_full, peers, **remap)
+            project(p, a, q, p.get("nq"), q_loc)
+            hdl.barrier(channel=0)
+        else:
+            kv_full = kv_all
+            project(p, a, kv, p.get("nk"), kv_loc)
+            work = gather(kv_loc, kv_full)
+            project(p, a, q, p.get("nq"), q_loc)
+            work.wait()
+        attend(kv_full, out)
+    return qkv_attend
+
+
 def sharded_temporal_qkv_attend(plan, kind, B, T_loc, V, Hp, Wp, D, heads, q_loc, peer_kv=None,
                                 kv_loc=None, kv_all=None, eps=1e-5):
     """`VTSelfAttentionBlock.run`'s qkv_attend for frame-sharded temporal attention (kind
@@ -121,19 +159,12 @@ def sharded_temporal_qkv_attend(plan, kind, B, T_loc, V, Hp, Wp, D, heads, q_loc
     mapping into local AND peer memory (fused scatter over NVLink, `peer_kv` a PeerKV whose
     buffers hold at least B*T*V*S x 2D), or through an all-gather (kv_loc, kv_all) — while
     the Q projection runs into q_loc; then every local query frame attends to all T frames
-    with the single-GPU key addressing."""
+    with the single-GPU key addressing.  V is the number of views this rank holds (all
+    views, or the V_loc of a view shard: the frame group exchanges the local views)."""
     S, T = Hp * Wp, plan.T
     # local rows -> rows of the unsharded layout: item = batch entry
     remap = dict(rows_per_item=T_loc * V * S, out_item_stride=T * V * S,
                  out_row_offset=plan.t_offset * V * S)
-
-    def project(p, a, w, nw, out, peer_out=None, **kw):
-        if p["qk_norm"]:
-            gemm(a, w, epilogue=_lib.EPI_QKNORM, out=out,
-                 q_norm_weight=nw, qk_region=D, qk_norm_regions=1,
-                 eps=eps, peer_out=peer_out, **kw)
-        else:
-            gemm(a, w, out=out, peer_out=peer_out, **kw)
 
     def attend(kv_all, out):
         if kind == "full":         # (b v) (t hw)
@@ -158,25 +189,41 @@ def sharded_temporal_qkv_attend(plan, kind, B, T_loc, V, Hp, Wp, D, heads, q_loc
                 kv_group_strides=[T * V * S, 1], seq_kv=T, inner_kv=1,
                 kv_stride_outer=V * S, kv_stride_inner=0)
 
-    def qkv_attend(p, a, out):
-        q, kv = p["qkv"].rows(0, D), p["qkv"].rows(D, 3 * D)
-        if peer_kv is not None:
-            # fused: the K,V GEMM epilogue scatters its tiles into every peer's
-            # gathered buffer over NVLink; one group barrier publishes them
-            kv_full, peers, hdl = peer_kv.next()
-            # the leading rows at this block's width (peers address their buffers the same way)
-            kv_full = kv_full.view(-1)[:B * T * V * S * 2 * D].view(B * T * V * S, 2 * D)
-            project(p, a, kv, p.get("nk"), kv_full, peers, **remap)
-            project(p, a, q, p.get("nq"), q_loc)
-            hdl.barrier(channel=0)
-        else:
-            kv_full = kv_all
-            project(p, a, kv, p.get("nk"), kv_loc)
-            work = plan.gather_frames_kv(kv_loc, kv_full, batch=B, async_op=True)
-            project(p, a, q, p.get("nq"), q_loc)
-            work.wait()
-        attend(kv_full, out)
-    return qkv_attend
+    def gather(kv_loc, kv_full):
+        return plan.gather_frames_kv(kv_loc, kv_full, batch=B, async_op=True)
+    return _sharded_qkv_attend(D, eps, B * T * V * S, remap, q_loc, attend, gather, peer_kv,
+                               kv_loc, kv_all)
+
+
+def sharded_crossview_qkv_attend(plan, items, Hp, Wp, D, heads, q_loc, mask, mask_div,
+                                 peer_kv=None, kv_loc=None, kv_all=None, eps=1e-5):
+    """`VTSelfAttentionBlock.run`'s qkv_attend for row-wise cross-view attention
+    "(bt v) (h w) -> (bt h) (v w)" on a view shard (plan.V_loc views from plan.v_offset of
+    plan.V): K,V of the local views go to the gathered buffer of the local frames
+    [items * V * S, 2D] (items = batch entries x local frames) in the unsharded view order,
+    through the epilogue remap (item = one (b, t), V_loc * S rows each) with a peer scatter
+    over the view group, or an all-gather over it (kv_loc, kv_all).  The local query views
+    then attend to all V views; query unit u reads row v_offset + u of the [B, V, V] view mask.
+    Without a mask an all-ones one is used: it selects the kernel the unsharded launch runs
+    on, and allows every view as no mask does."""
+    S, V, V_loc, v_off = Hp * Wp, plan.V, plan.V_loc, plan.v_offset
+    remap = dict(rows_per_item=V_loc * S, out_item_stride=V * S, out_row_offset=v_off * S)
+    if mask is None:
+        mask = torch.ones(1, V, V, dtype=torch.uint8, device=q_loc.device)
+        mask_div = items
+
+    def attend(kv_all, out):
+        _ops.attention(
+            q_loc, out, D=D, heads=heads, group_dims=[items, Hp],
+            group_strides=[V_loc * S, Wp], seq=V_loc * Wp, inner=Wp, stride_outer=S,
+            stride_inner=1, mask=mask, mask_div=mask_div, mask_q_offset=v_off,
+            kv=kv_all, k_col=0, v_col=D, kv_group_strides=[V * S, Wp], seq_kv=V * Wp,
+            inner_kv=Wp, kv_stride_outer=S, kv_stride_inner=1)
+
+    def gather(kv_loc, kv_full):
+        return plan.gather_views_kv(kv_loc, kv_full, items=items, async_op=True)
+    return _sharded_qkv_attend(D, eps, items * V * S, remap, q_loc, attend, gather, peer_kv,
+                               kv_loc, kv_all)
 
 
 class VTSelfAttentionBlock(torch.nn.Module):

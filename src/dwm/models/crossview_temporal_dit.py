@@ -32,7 +32,7 @@ from .. import _compat
 from . import adapters as _adapters
 from .crossview_temporal import (
     AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward,
-    sharded_temporal_qkv_attend)
+    sharded_crossview_qkv_attend, sharded_temporal_qkv_attend)
 from .packing import (
     FP8, Operand, fp32, fp8_bytes_saved, gemm, layernorm, pack_linear, requantize)
 
@@ -416,8 +416,9 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
     def _conditions(self, B, T, V, Hp, Wp, t_offset, T_total,
                     encoder_hidden_states, pooled_projections,
                     condition_image_tensor, added_time_ids, disable_crossview,
-                    disable_temporal, crossview_attention_mask):
-        key = (B, T, V, Hp, Wp, t_offset, T_total,
+                    disable_temporal, crossview_attention_mask, v_offset=0, V_total=None):
+        V_total = V if V_total is None else V_total
+        key = (B, T, V, Hp, Wp, t_offset, T_total, v_offset, V_total,
                self._tkey(encoder_hidden_states), self._tkey(pooled_projections),
                self._tkey(condition_image_tensor), self._tkey(added_time_ids),
                self._tkey(disable_crossview), self._tkey(disable_temporal),
@@ -429,11 +430,11 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         refs = (encoder_hidden_states, pooled_projections, condition_image_tensor,
                 added_time_ids, disable_crossview, disable_temporal, crossview_attention_mask)
         if self.__dict__.pop("_ring_shift", False) and self._ring_applicable(
-                B, T, V, Hp, Wp, t_offset, T_total, condition_image_tensor):
+                B, T, V, Hp, Wp, t_offset, T_total, condition_image_tensor, v_offset, V_total):
             cd = self._conditions_shifted(
                 B, T, V, Hp, Wp, t_offset, T_total, encoder_hidden_states, pooled_projections,
                 condition_image_tensor, added_time_ids, disable_crossview, disable_temporal,
-                crossview_attention_mask)
+                crossview_attention_mask, v_offset, V_total)
             self._cond_key, self._cond, self._cond_refs = key, cd, refs
             return cd
         pk, dt, D = self._pk, self._pk["dtype"], self.inner_dim
@@ -465,9 +466,12 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
 
         item_t = (torch.arange(T, device=dev) + t_offset).view(1, T, 1)\
             .expand(B, T, V).reshape(-1)
-        item_v = torch.arange(V, device=dev).view(1, 1, V)\
+        # a view shard holds views v_offset ... v_offset + V - 1 of V_total: its view index
+        # embeddings are rows of the table over all views
+        item_v = (torch.arange(V, device=dev) + v_offset).view(1, 1, V)\
             .expand(B, T, V).reshape(-1)
-        cd["_geom"], cd["_view_cam"] = (B, T, V, Hp, Wp, t_offset, T_total), view_cam
+        cd["_geom"] = (B, T, V, Hp, Wp, t_offset, T_total, v_offset, V_total)
+        cd["_view_cam"] = view_cam
         if self.enable_temporal:
             tabs = index_table(T_total, pk["tpe"])
             cd["_tabs_t"] = tabs
@@ -483,7 +487,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
             cd["t_alpha"] = [m.batch_alpha(B, dis.flatten().to(dev), dev)
                              for m in self.time_mixers]
         if self.enable_crossview:
-            tabs = index_table(V, pk["vpe"])
+            tabs = index_table(V_total, pk["vpe"])
             cd["_tabs_v"] = tabs
             cd["vemb_tab"] = []
             for tab in tabs:
@@ -507,16 +511,16 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         return cd
 
     # -- streaming ring update of the step-invariant cache (opt-in, SURVEY.md §8(f)2) -----------
-    def _ring_applicable(self, B, T, V, Hp, Wp, t_offset, T_total, image):
+    def _ring_applicable(self, B, T, V, Hp, Wp, t_offset, T_total, image, v_offset, V_total):
         """T frames from t_offset of a T_total-frame window: the whole window on one GPU, or
-        a frame shard (`ShardPlan`) of it."""
+        a frame and / or view shard (`ShardPlan`) of it."""
         old = self._cond
         return old is not None and T > 1 and \
-            old.get("_geom") == (B, T, V, Hp, Wp, t_offset, T_total) and \
+            old.get("_geom") == (B, T, V, Hp, Wp, t_offset, T_total, v_offset, V_total) and \
             (image is None or image.shape[1] == T)
 
     def _conditions_shifted(self, B, T, V, Hp, Wp, t_offset, T_total, ehs, pooled, image, ids,
-                            dis_cv, dis_t, mask):
+                            dis_cv, dis_t, mask, v_offset, V_total):
         """The FIFO moved on by one frame: every per-item entry of the cached condition set is
         the old one shifted by a frame, only the last frame's entries (context embedding, pooled
         text MLP, camera embedding, ImageAdapter residuals) are computed.  The index-embedding
@@ -529,7 +533,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         self._cond_key = None
         one = lambda t: None if t is None else t[:, T - 1:]          # noqa: E731
         cd1 = self._conditions(B, 1, V, Hp, Wp, t_offset + T - 1, T_total, one(ehs), one(pooled),
-                               one(image), one(ids), dis_cv, dis_t, mask)
+                               one(image), one(ids), dis_cv, dis_t, mask, v_offset, V_total)
         self._cond_key, self._cond = saved
 
         def shift(o, n):
@@ -546,7 +550,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         dev = cd["c0"].device
         item_t = (torch.arange(T, device=dev) + t_offset).view(1, T, 1)\
             .expand(B, T, V).reshape(-1)
-        item_v = torch.arange(V, device=dev).view(1, 1, V).expand(B, T, V).reshape(-1)
+        item_v = (torch.arange(V, device=dev) + v_offset).view(1, 1, V).expand(B, T, V).reshape(-1)
         if self.enable_temporal:
             cd["temb_tab"] = []
             for tab in old["_tabs_t"]:
@@ -637,6 +641,32 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
             plan, self.temporal_attention_type, B, T_loc, V, Hp, Wp, D, heads, ws["q_loc"],
             peer_kv=ws["peer_kv"], kv_loc=ws.get("kv_loc"), kv_all=ws.get("kv_all"))
 
+    def _crossview_qkv_attend_sharded(self, B, T, V_loc, Hp, Wp, ws, mask):
+        """Row-wise cross-view attention of a view shard (`sharded_crossview_qkv_attend`): local
+        query views against the K,V of all views, gathered over the view group, with its
+        buffers kept in the step workspace for the input geometry."""
+        plan = self.shard
+        if self.crossview_attention_type != "rowwise":
+            raise NotImplementedError(
+                "crossview {!r} attention under a view shard: only 'rowwise' (the CTSD "
+                "configs) is sharded".format(self.crossview_attention_type))
+        S, D, heads = Hp * Wp, self.inner_dim, self.heads
+        rows, rows_full = B * T * V_loc * S, B * T * plan.V * S
+        dt, dev = ws["a16"].dtype, ws["a16"].device
+        if ws.get("cv_geom") != (rows, rows_full):
+            ws["cv_geom"] = (rows, rows_full)
+            ws["cv_q_loc"] = torch.empty(rows, D, device=dev, dtype=dt)
+            ws["cv_peer_kv"] = None
+            if plan.use_peer_scatter:
+                from opendwm_b200.sharding import PeerKV
+                ws["cv_peer_kv"] = PeerKV(plan, rows_full, 2 * D, dt, dev, axis="v")
+            else:
+                ws["cv_kv_loc"] = torch.empty(rows, 2 * D, device=dev, dtype=dt)
+                ws["cv_kv_all"] = torch.empty(rows_full, 2 * D, device=dev, dtype=dt)
+        return sharded_crossview_qkv_attend(
+            plan, B * T, Hp, Wp, D, heads, ws["cv_q_loc"], mask, T,
+            peer_kv=ws["cv_peer_kv"], kv_loc=ws.get("cv_kv_loc"), kv_all=ws.get("cv_kv_all"))
+
     # -- one JointTransformerBlock ----------------------------------------------------------
     def _joint_block(self, b, ws, N, S, L, residual):
         D, heads = self.inner_dim, self.heads
@@ -712,14 +742,16 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         self, sample, timestep, encoder_hidden_states, pooled_projections,
         condition_image_tensor=None, disable_crossview=None,
         disable_temporal=None, crossview_attention_mask=None,
-        added_time_ids=None, t_offset=0, T_total=None, cfg_repeat=1
+        added_time_ids=None, t_offset=0, T_total=None, cfg_repeat=1, v_offset=0, V_total=None
     ):
         """Runs the noise-predict forward and returns the proj_out tokens
         fp32 [B*T*V*S, p*p*C] (column = (py*p+px)*C + c) plus the geometry; the
         fused CFG/Euler kernel and `forward` un-patchify from this.
         `cfg_repeat=2`: `sample` / `timestep` hold ONE copy of the batch and stand for
         `torch.cat([x, x])` (reference ctsd.py:2058-2063) — the patchify and timestep kernels
-        write both halves, no concatenated copy is materialised."""
+        write both halves, no concatenated copy is materialised.
+        A frame / view shard of a ShardPlan (`self.shard`) passes the frames from t_offset of
+        T_total and the views from v_offset of V_total it holds."""
         if self._pk is None:
             self._pack()
         pk = self._pk
@@ -735,7 +767,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         cd = self._conditions(
             B, T, V, Hp, Wp, t_offset, T_total, encoder_hidden_states,
             pooled_projections, condition_image_tensor, added_time_ids,
-            disable_crossview, disable_temporal, crossview_attention_mask)
+            disable_crossview, disable_temporal, crossview_attention_mask, v_offset, V_total)
         L = cd["L"]
         ws = self._workspace(N, S, L, sample.device, dt)
 
@@ -767,6 +799,9 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
         residuals = list(cd["residuals"])
         cv_attend = self._crossview_attend(B, T, V, Hp, Wp, cd.get("mask")) \
             if self.enable_crossview else None
+        cv_sharded = None
+        if self.enable_crossview and self.shard is not None and self.shard.v_ways > 1:
+            cv_sharded = self._crossview_qkv_attend_sharded(B, T, V, Hp, Wp, ws, cd.get("mask"))
         tp_attend = self._temporal_attend(B, T, V, Hp, Wp) \
             if self.enable_temporal else None
         tp_sharded = None
@@ -790,7 +825,7 @@ class DiTCrossviewTemporalConditionModel(_compat.SD3Transformer2DModelMarker):
                 k = self.crossview_block_layers.index(i)
                 self.crossview_transformer_blocks[k].run(
                     pk["cv"][k], ws["x"], cd["vemb_tab"][k], S, ws, cv_attend,
-                    cd["v_alpha"][k], T * V * S)
+                    cd["v_alpha"][k], T * V * S, qkv_attend=cv_sharded)
                 if trace is not None:
                     trace(("crossview", i), ws["x"])
 

@@ -23,7 +23,7 @@ from .. import _compat
 from . import adapters as _adapters
 from .crossview_temporal import (
     AlphaBlender, ParamGroup, VTSelfAttentionBlock, make_attention, make_feed_forward,
-    sharded_temporal_qkv_attend)
+    sharded_crossview_qkv_attend, sharded_temporal_qkv_attend)
 from .packing import (
     FP8, Operand, conv, gemm, layernorm, pack_conv, pack_linear, pack_norm, requantize)
 
@@ -416,27 +416,36 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
     def _frame_sharded(self):
         return self.shard is not None and self.shard.t_ways > 1
 
+    def _view_sharded(self):
+        return self.shard is not None and self.shard.v_ways > 1
+
     def _peer_buffers(self, geo, H, W):
         """Symmetric-memory K,V (PeerKV) and temporal-conv operand (PeerHalo) buffers of the
-        frame group, sized once per input geometry for the largest level (channels x pixels)
-        and shared by all temporal blocks in forward order: creating them is collective, so it
-        must not happen per block or per step.  (None, None) with DWM_PEER_SCATTER=0."""
+        frame group, and the K,V buffers (PeerKV) of the view group, sized once per input
+        geometry for the largest level (channels x pixels) and shared by all temporal /
+        cross-view blocks in forward order: creating them is collective, so it must not happen
+        per block or per step.  None for a group the plan does not split, and all None with
+        DWM_PEER_SCATTER=0."""
         plan = self.shard
         dt = self._pk["dtype"]
         key = (id(plan), geo, H, W, dt)
         if self._peer_key != key:
-            self._peer, self._peer_key = (None, None), key
+            self._peer, self._peer_key = (None, None, None), key
             if plan.use_peer_scatter:
                 from opendwm_b200.sharding import PeerHalo, PeerKV
-                B, _, V = geo
+                B, T, V = geo
                 widest, h, w = 0, H, W
                 for c in self.config["block_out_channels"]:
                     widest = max(widest, c * h * w)
                     h, w = (h + 1) // 2, (w + 1) // 2
                 dev = self.conv_in.weight.device
+                frames = self._frame_sharded()
                 self._peer = (
-                    PeerKV(plan, B * plan.T * V * widest, 2, dt, dev),
-                    PeerHalo(plan, B * V * (max(plan.counts) + 2) * widest * dt.itemsize, dev))
+                    PeerKV(plan, B * plan.T * V * widest, 2, dt, dev) if frames else None,
+                    PeerHalo(plan, B * V * (max(plan.counts) + 2) * widest * dt.itemsize, dev)
+                    if frames else None,
+                    PeerKV(plan, B * T * plan.V * widest, 2, dt, dev, axis="v")
+                    if self._view_sharded() else None)
         return self._peer
 
     def _norm_act_shard(self, x5, g):
@@ -554,8 +563,12 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
             item_v = torch.arange(V, device=dev).view(1, 1, V).expand(B, T, V).reshape(-1)
             item_t = torch.arange(T, device=dev).view(1, T, 1).expand(B, T, V).reshape(-1)
             if "vpe" in p:
-                tabs["v"] = self._index_table(V, p["vpe"], tm.in_channels, dev, dt)[item_v]\
-                    .contiguous()
+                if self._view_sharded():      # view index within all views
+                    tab = self._index_table(self.shard.V, p["vpe"], tm.in_channels, dev, dt)
+                    item_v = item_v + self.shard.v_offset
+                else:
+                    tab = self._index_table(V, p["vpe"], tm.in_channels, dev, dt)
+                tabs["v"] = tab[item_v].contiguous()
             if "tpe" in p:
                 if self._frame_sharded():     # frame index within the whole window
                     tab = self._index_table(self.shard.T, p["tpe"], tm.in_channels, dev, dt)
@@ -577,6 +590,21 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                 plan, "rowwise" if tm.enable_rowwise_temporal else "pointwise", B, T, V, H, W,
                 inner, heads, torch.empty(rows, inner, device=dev, dtype=dt), peer_kv=peer_kv,
                 kv_loc=kv_loc, kv_all=kv_all)
+        cv_sharded = None
+        if "cv" in p and self._view_sharded():
+            if not tm.enable_rowwise_crossview:
+                raise NotImplementedError(
+                    "point-wise cross-view attention under a view shard: only row-wise "
+                    "cross-view attention is sharded")
+            plan, rows = self.shard, N * S
+            peer_kv = self._peer[2]
+            kv_loc = kv_all = None
+            if peer_kv is None:
+                kv_loc = torch.empty(rows, 2 * inner, device=dev, dtype=dt)
+                kv_all = torch.empty(B * T * plan.V * S, 2 * inner, device=dev, dtype=dt)
+            cv_sharded = sharded_crossview_qkv_attend(
+                plan, B * T, H, W, inner, heads, torch.empty(rows, inner, device=dev, dtype=dt),
+                cd["mask"], T, peer_kv=peer_kv, kv_loc=kv_loc, kv_all=kv_all)
         for li, bp in enumerate(p["blocks"]):
             # --- spatial BasicTransformerBlock: self-attn, cross-attn to text, GEGLU FF
             n = bp["n1"]
@@ -619,7 +647,8 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
                                        stride_outer=S, stride_inner=0)
                 tm.crossview_transformer_blocks[li].run(
                     p["cv"][li], h, tabs["v"], S, ws, attend,
-                    tm.view_mixer.batch_alpha(B, cd["dis_cv"]["t"], dev), T * V * S)
+                    tm.view_mixer.batch_alpha(B, cd["dis_cv"]["t"], dev), T * V * S,
+                    qkv_attend=cv_sharded)
             # --- temporal block
             if "tp" in p and not cd["dis_t"]["all"]:
                 if tm.enable_rowwise_temporal:    # (b v h) x (t w)
@@ -688,8 +717,9 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
 
     def _conditions(self, geo, H, W, encoder_hidden_states, condition_image_tensor,
                     added_time_ids, disable_crossview, disable_temporal, mask):
-        # the frame-index tables depend on where a frame shard sits in the window
-        shard = (self.shard.T, self.shard.t_offset) if self._frame_sharded() else None
+        # the frame / view index tables depend on where a shard sits in the window
+        shard = (self.shard.T, self.shard.t_offset, self.shard.V, self.shard.v_offset) \
+            if self._frame_sharded() or self._view_sharded() else None
         key = (geo, H, W, shard) + tuple(self._tkey(t) for t in (
             encoder_hidden_states, condition_image_tensor, added_time_ids, disable_crossview,
             disable_temporal, mask))
@@ -756,10 +786,13 @@ class UNetCrossviewTemporalConditionModel(_compat.UNetSpatioTemporalConditionMod
         N, geo, dev = B * T * V, (B, T, V), sample.device
         if self._ws8_key != (B, T, V, H, W):     # one live E4M3 workspace
             self._ws8, self._ws8_key = {}, (B, T, V, H, W)
-        if self._frame_sharded():
-            if T != self.shard.T_loc:
-                raise ValueError("sample holds {} frames, the ShardPlan's shard {}".format(
-                    T, self.shard.T_loc))
+        if self._frame_sharded() and T != self.shard.T_loc:
+            raise ValueError("sample holds {} frames, the ShardPlan's shard {}".format(
+                T, self.shard.T_loc))
+        if self._view_sharded() and V != self.shard.V_loc:
+            raise ValueError("sample holds {} views, the ShardPlan's shard {}".format(
+                V, self.shard.V_loc))
+        if self._frame_sharded() or self._view_sharded():
             self._peer_buffers(geo, H, W)
         cd = self._conditions(geo, H, W, encoder_hidden_states, condition_image_tensor,
                               added_time_ids, disable_crossview, disable_temporal,

@@ -405,7 +405,9 @@ class CrossviewTemporalSD:
             conditions.get("added_time_ids"),
             t_offset=0 if plan is None else plan.t_offset,
             T_total=None if plan is None else plan.T,
-            cfg_repeat=2 if (do_cfg and not split_cfg) else 1)
+            cfg_repeat=2 if (do_cfg and not split_cfg) else 1,
+            v_offset=0 if plan is None else plan.v_offset,
+            V_total=None if plan is None else plan.V)
         if split_cfg:   # exchange the branch predictions inside the CFG pair
             both = getattr(self, "_cfg_tokens", None)
             if both is None or both.shape[0] != 2 * tokens.shape[0]:
@@ -442,6 +444,9 @@ class CrossviewTemporalSD:
             # the peer K,V buffers alternate per temporal block; a captured step with an odd
             # number of blocks would end and restart on the same buffer (no barrier in between)
             sharded = True
+        if self.sharding is not None and self.sharding.v_ways > 1 and \
+                len(getattr(self.model, "crossview_block_layers", None) or ()) % 2 == 1:
+            sharded = True          # the same for the view group's cross-view buffers
         if sharded or stateful:
             return self.denoise_step(latents, conditions, idx, timesteps, in_range)
         key = (latents.data_ptr(), tuple(latents.shape), idx is None, in_range is None,
@@ -585,12 +590,12 @@ class CrossviewTemporalSD:
         inject = (not df_mode) and image_latents is not None and \
             reference_frame_count > 0
         # end-to-end sharding (opendwm_b200.sharding.ShardPlan in self.sharding): every rank
-        # builds the full noise / conditions (same generator seed), keeps its CFG branch and
-        # frames for the steps, and the window is re-assembled before the decode
+        # builds the full noise / conditions (same generator seed), keeps its CFG branch,
+        # frames and views for the steps, and the window is re-assembled before the decode
         plan = self.sharding
-        fs = slice(0, T)
+        fs, vs = slice(0, T), slice(None)
         if plan is not None:
-            fs = plan.frame_slice()
+            fs, vs = plan.frame_slice(), plan.view_slice()
             conditions = plan.local_conditions(
                 conditions, cfg_doubled="guidance_scale" in self.inference_config)
             latents = plan.local_latents(latents)
@@ -618,9 +623,10 @@ class CrossviewTemporalSD:
                 timesteps[:, :reference_frame_count] = 0
                 n_loc = max(0, min(reference_frame_count, fs.stop) - fs.start)
                 if n_loc > 0:
-                    latents[:, :n_loc] = image_latents[:, fs.start:fs.start + n_loc].to(latents)
+                    latents[:, :n_loc] = \
+                        image_latents[:, fs.start:fs.start + n_loc, vs].to(latents)
             if plan is not None:
-                idx, timesteps = idx[:, fs].contiguous(), timesteps[:, fs].contiguous()
+                idx, timesteps = idx[:, fs, vs].contiguous(), timesteps[:, fs, vs].contiguous()
                 in_range = None if in_range is None else in_range[fs].contiguous()
             step(latents, conditions, idx, timesteps, in_range)
         if plan is not None:
@@ -884,10 +890,14 @@ class StreamingCrossviewTemporalSD(CrossviewTemporalSD):
         stop_timestep = stop_timestep or steps
         plan = self._streaming_plan()
         conditions, fs, decode, work = self.conditions, None, self.decode_latents, latents
+        V_work = V
         if plan is not None:
             if plan.T != T:
                 raise ValueError("the ShardPlan splits {} frames, the FIFO holds {}".format(
                     plan.T, T))
+            if plan.V is not None and plan.V != V:
+                raise ValueError("the ShardPlan splits {} views, the FIFO holds {}".format(
+                    plan.V, V))
             # sliced once per condition update: the flush reuses one condition set, and the
             # model's condition cache is keyed by tensor address
             if self._local_conditions is None or self._local_conditions[0] is not plan:
@@ -895,11 +905,12 @@ class StreamingCrossviewTemporalSD(CrossviewTemporalSD):
                     self.conditions, cfg_doubled="guidance_scale" in self.inference_config))
             conditions, fs = self._local_conditions[1], plan.frame_slice()
             work = plan.local_latents(latents)
+            V_work = work.shape[2]
             if self.vae is not None:
                 decode = lambda t: plan.split_call(self.decode_latents, t)  # noqa: E731
         for i in range(start_timestep, stop_timestep):
             idx, timesteps, in_range = self._df_step_tensors(
-                i, T, spi, take_time, B, V, frames=fs)
+                i, T, spi, take_time, B, V_work, frames=fs)
             self.denoise_step(work, conditions, idx, timesteps, in_range)
         if plan is not None:
             # unsharded, the steps update `latents` in place, and an fp32 FIFO is `latents`

@@ -6,7 +6,15 @@
 Every rank builds the same seeded small DiT, runs diffusion-forcing denoise steps with the
 CFG x frame sharding plan, and the gathered latents are compared with an unsharded run of
 the same steps on rank 0.  Exit code 0 = match.  `--unet` checks the CTSD-2.1 UNet instead
-(`unet_main`)."""
+(`unet_main`).
+
+`--views` adds the view axis to the plan (CFG x views x frames, the split `ShardPlan` picks, or
+`--view-ways K`): cross-view blocks then gather their K,V over the view group.
+
+`--count [--world N] [--frames T] [--views V]` runs no GPU work: it prints, for the DiT plans of
+N GPUs, the K,V exchanges per denoise step and the bytes each rank sends in them (CTSD-3.5 DiT:
+6 cross-view and 12 temporal blocks, D = 1536, 16 x 28 patches per view, 16-bit K,V), for
+config 2's image window (T = 1) and config 5's 5 latent frames by default."""
 import os
 import sys
 
@@ -16,6 +24,39 @@ for p in (ROOT, os.path.join(ROOT, "src"), os.path.join(ROOT, "tests")):
 
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
+
+
+def _arg(name, default):
+    return int(sys.argv[sys.argv.index(name) + 1]) if name in sys.argv else default
+
+
+def count_main():
+    """--count: K,V exchanges per step and bytes sent per rank, from shapes (no GPU)."""
+    from opendwm_b200.sharding import ShardPlan
+    D, S, n_cv, n_tp, eb = 1536, 16 * 28, 6, 12, 2
+    worlds = [_arg("--world", 0)] if "--world" in sys.argv else [2, 4, 8]
+    windows = [(_arg("--frames", 5), _arg("--views", 6))] if "--frames" in sys.argv else \
+        [(1, 6), (5, 6)]
+    for T, V in windows:
+        for world in worlds:
+            for views in (None, V):
+                try:
+                    p = ShardPlan(world, 0, T, make_groups=False, views=views)
+                except ValueError as e:
+                    print("count T=%d V=%d world=%d views=%s: %s" % (T, V, world, views, e))
+                    continue
+                V_loc = V if views is None else max(p.v_counts)
+                T_loc = max(p.counts)
+                rows = T_loc * V_loc * S                     # largest shard, one CFG branch
+                kv = rows * 2 * D * eb
+                cv = n_cv if p.v_ways > 1 else 0
+                tp = n_tp if p.t_ways > 1 else 0
+                sent = cv * kv * (p.v_ways - 1) + tp * kv * (p.t_ways - 1)
+                print("count T=%d V=%d world=%d plan=%s largest_shard_items=%d "
+                      "crossview_exchanges=%d temporal_exchanges=%d cfg_exchanges=%d "
+                      "MB_sent_per_rank_per_step=%.1f" % (
+                          T, V, world, p.parallelism, T_loc * V_loc, cv, tp,
+                          1 if p.cfg_ways > 1 else 0, sent / 1e6))
 
 
 def main():
@@ -30,7 +71,10 @@ def main():
     dist.init_process_group("nccl", device_id=torch.device("cuda", torch.cuda.current_device()))
     V = 3
     use_cfg = os.environ.get("SHARD_CFG", "1") != "0"
-    t_ways = world // (2 if (use_cfg and world >= 2) else 1)
+    views = V if "--views" in sys.argv else None
+    view_ways = _arg("--view-ways", None)
+    t_ways = ShardPlan(world, 0, 64, cfg=use_cfg, make_groups=False, views=views,
+                       view_ways=view_ways).t_ways
     # (frames, temporal attention type): 8 = even shards; 5 / 11 / 19 = the uneven shards of
     # BASELINE configs 5 and 3 (19 with row-wise temporal attention as in config 3); full
     # temporal attention on even and uneven shards
@@ -74,13 +118,14 @@ def main():
             lat = latents0.clone() if plan is None else plan.local_latents(latents0)
             c = cond if plan is None else plan.local_conditions(cond, cfg_doubled=True)
             fs = slice(0, T) if plan is None else plan.frame_slice()
+            vs = slice(None) if plan is None else plan.view_slice()
             for i in (steps - 3, steps - 2, steps - 1):
                 idx, ts, in_range = pipe._df_step_tensors(i, T, spi, 0, 1, V)
-                pipe.denoise_step(lat, c, idx[:, fs].contiguous(), ts[:, fs].contiguous(),
-                                  in_range[fs].contiguous())
+                pipe.denoise_step(lat, c, idx[:, fs, vs].contiguous(),
+                                  ts[:, fs, vs].contiguous(), in_range[fs].contiguous())
             return lat if plan is None else plan.gather_latents(lat)
 
-        plan = ShardPlan(world, rank, T, cfg=use_cfg)
+        plan = ShardPlan(world, rank, T, cfg=use_cfg, views=views, view_ways=view_ways)
         sharded = run(plan)
         ref = run(None)
         err = ((sharded - ref).abs().max() / ref.abs().max()).item()
@@ -91,11 +136,11 @@ def main():
         worst = max(worst, t[0].item())
         all_equal = all_equal and t[1].item() == 0.0 and t[2].item() == 0.0
         if rank == 0:
-            print("shard_check world=%d plan=%s T=%d shards=%s temporal=%s peer_scatter=%s "
-                  "bit_identical=%s max_rel_err=%.3e (latents moved %.3f)" % (
-                      world, plan.parallelism, T, plan.counts, kind,
-                      plan.use_peer_scatter and plan.t_ways > 1, t[1].item() == 0.0,
-                      t[0].item(), moved), flush=True)
+            print("shard_check world=%d plan=%s T=%d shards=%s view_shards=%s temporal=%s "
+                  "peer_scatter=%s bit_identical=%s max_rel_err=%.3e (latents moved %.3f)" % (
+                      world, plan.parallelism, T, plan.counts, plan.v_counts, kind,
+                      plan.use_peer_scatter and (plan.t_ways > 1 or plan.v_ways > 1),
+                      t[1].item() == 0.0, t[0].item(), moved), flush=True)
         del pipe, model
         torch.cuda.empty_cache()
     dist.destroy_process_group()
@@ -148,4 +193,9 @@ def unet_main():
 
 
 if __name__ == "__main__":
-    unet_main() if "--unet" in sys.argv else main()
+    if "--count" in sys.argv:
+        count_main()
+    elif "--unet" in sys.argv:
+        unet_main()
+    else:
+        main()

@@ -12,6 +12,9 @@ call pair plus the copy of the decoded views to the host, synchronised on both s
 denoise steps, the condition-cache ring update, the FIFO all-gather and the item-parallel VAE
 decode.
 
+`--views` attaches `ShardPlan(N, rank, 16, cfg=True, views=6)` instead (the split of the view
+and frame axes the plan picks, or `--view-ways K`).
+
 `--check`: the FIFO latents after every call are also kept on rank 0, which then streams the
 same frames without a plan and compares them bit for bit.
 
@@ -76,6 +79,9 @@ def main():
                     help="compare the FIFO after every call with an unsharded stream on rank 0")
     ap.add_argument("--dtype", choices=["bf16", "fp16"], default="fp16")
     ap.add_argument("--small", action="store_true", help="4-layer model, 4 frames (smoke)")
+    ap.add_argument("--views", action="store_true",
+                    help="plan with the view axis (CFG x views x frames)")
+    ap.add_argument("--view-ways", type=int, default=None, help="force the view split")
     args = ap.parse_args()
 
     import bench
@@ -123,7 +129,8 @@ def main():
         pipe.sharding = plan
         return pipe
 
-    plan = ShardPlan(world, rank, T, cfg=True)
+    plan = ShardPlan(world, rank, T, cfg=True, views=V if args.views else None,
+                     view_ways=args.view_ways)
     secs, fifo = _stream(pipeline(plan), cfg, T, args.frames, args.check, timed=True)
     mean = sum(secs) / len(secs)
     slowest = mean
