@@ -305,7 +305,8 @@ int dwm_b200_euler_step_by_indices(const float* model_output, float* sample, int
  * spatial zero padding kh/2, kw/2; no implicit temporal padding.  c_out must be a multiple
  * of 32 (pad the weight rows); tiles of 256 / 128 / 64 / 32 output channels.  Epilogues: DWM_EPI_STORE (16-bit,
  * bias + act), DWM_EPI_F32, DWM_EPI_RESID (fp32: acc + bias + resid).  Opt-in E4M3 x and
- * weight with per-volume / per-channel scales (a_scale, w_scale below), RESID only.
+ * weight with per-volume / per-channel scales (a_scale, w_scale below): RESID, and F32 when
+ * c_out is a multiple of 128 (the VAE ResNet conv1).
  * Replaces diffusers CogVideoXCausalConv3d / CogVideoXUpsample3D.conv inside
  * AutoencoderKLCogVideoX.decode (called at ctsd.py:1634-1640, 1615-1617) and the
  * AdapterResnetBlock 3x3 convs (adapters.py:20). */
@@ -334,7 +335,8 @@ typedef struct dwm_conv_args {
   int64_t ldx;
   const float* alpha;
   int64_t rows_per_batch;
-  /* FP8 (dtype == DWM_E4M3; epilogue DWM_EPI_RESID only): x and weight are E4M3, with
+  /* FP8 (dtype == DWM_E4M3; epilogue DWM_EPI_RESID, or DWM_EPI_F32 with c_out % 128 == 0):
+   * x and weight are E4M3, with
    * a_scale fp32 [nb] (one scale per VOLUME: every tap of an output pixel reads the same
    * volume) and w_scale fp32 [c_out] (one per output channel, over all taps and input
    * channels; 8-byte aligned).  The fp32 accumulator is multiplied by a_scale[nb] *
@@ -379,6 +381,24 @@ int dwm_b200_groupnorm_silu_e4m3(const float* x, int64_t nb, int64_t T, int64_t 
                                  int groups, const double* sums, float eps, const float* gamma,
                                  const float* beta, int apply_silu, void* out, int64_t out_T,
                                  int64_t out_t0, float* out_scale, dwm_stream_t stream);
+/* SpatialNorm3D(+SiLU) with an E4M3 output, the operand of an FP8 causal dwm_b200_conv of the
+ * CogVideoX decoder: the values y of dwm_b200_spatialnorm_silu (zy / zb and the latent frame map
+ * included), quantized with ONE scale per volume n by the rule of dwm_b200_groupnorm_silu_e4m3,
+ * into frames [out_t0, out_t0 + T) of out E4M3 [nb, out_T, H, W, C].  The causal-conv cache:
+ * tail_in (16-bit [nb, 2, H, W, C] of type tail_dtype, or NULL) is the previous chunk's cached
+ * tail; the volume's amax covers it and y, and it is quantized with that scale into frames
+ * out_t0 - 2, out_t0 - 1 (out_t0 >= 2).  Without tail_in those frames are left as they are (the
+ * caller copies frame out_t0's bytes there: they share the scale).  tail_out (same layout, may
+ * be tail_in) receives the next chunk's cache: the operand's last two frames in 16 bit, y
+ * rounded to tail_dtype or, for T = 1, tail_in's frame 1 (else y's replica) and y.  Passes:
+ * amax, quantize, scale; out_scale (fp32 [nb]) is the amax scratch, so nothing is allocated.
+ * C must be a multiple of 16. */
+int dwm_b200_spatialnorm_silu_e4m3(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C,
+                                   int groups, const double* sums, float eps, const float* gamma,
+                                   const float* beta, const float* zy, const float* zb, int Tz, int hz,
+                                   int wz, int apply_silu, void* out, int64_t out_T, int64_t out_t0,
+                                   float* out_scale, const void* tail_in, void* tail_out, int tail_dtype,
+                                   dwm_stream_t stream);
 /* Frame-shard GroupNorm(+SiLU) of the temporal ResBlock convolutions: x holds T of a window's
  * frames and `sums` (double [nb, groups, 2]) the statistics already summed over the window's
  * `stat_frames` frames, so mean and variance use stat_frames*H*W*C/groups samples.  out is the

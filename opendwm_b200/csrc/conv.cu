@@ -11,7 +11,8 @@
 // T2I-adapter 3x3 convs and the UNet ResBlock convs.  Epilogues are the GEMM ones (bias/act
 // store, fp32 residual).
 //
-// FP8 (opt-in, RESID epilogue only): E4M3 activations with ONE fp32 scale per volume nb and
+// FP8 (opt-in; RESID epilogue, and F32 at C_out tiles of 128 / 256 for the VAE ResNet conv1):
+// E4M3 activations with ONE fp32 scale per volume nb and
 // E4M3 weights with one scale per output channel (over all taps and input channels).  A
 // per-pixel scale could not be factored out of a sum over taps that read different pixels;
 // a volume scale can, because tiles never cross volumes and the padding is zero.  A stage is
@@ -286,6 +287,15 @@ static int conv_pick_bn(const dwm_conv_args* a, cudaStream_t s) {
   return -1;
 }
 
+// E4M3 with the fp32 store (the VAE ResNet conv1): only the C_out tiles the VAE widths
+// (128 / 256 / 512) select are instantiated
+static int conv_pick_bn_e4m3_f32(const dwm_conv_args* a, cudaStream_t s) {
+  if (a->c_out % 256 == 0) return launch_conv<__nv_fp8_e4m3, __nv_bfloat16, DWM_EPI_F32, 256>(a, s);
+  if (a->c_out % 128 == 0) return launch_conv<__nv_fp8_e4m3, __nv_bfloat16, DWM_EPI_F32, 128>(a, s);
+  set_last_error("dwm_b200_conv: E4M3 with DWM_EPI_F32 needs C_out %% 128 == 0; got %lld", (long long)a->c_out);
+  return -1;
+}
+
 template <typename T>
 static int conv_pick_epi(const dwm_conv_args* a, cudaStream_t s) {
   switch (a->epilogue) {
@@ -329,13 +339,14 @@ extern "C" int dwm_b200_conv(const dwm_conv_args* a, dwm_stream_t stream) {
   if (a->dtype == DWM_BF16) return conv_pick_epi<__nv_bfloat16>(a, s);
   if (a->dtype == DWM_F16) return conv_pick_epi<__half>(a, s);
   if (a->dtype == DWM_E4M3) {
-    DWM_REQUIRE(a->epilogue == DWM_EPI_RESID, "dwm_b200_conv: E4M3 operands need epilogue DWM_EPI_RESID, got %d",
-                a->epilogue);
+    DWM_REQUIRE(a->epilogue == DWM_EPI_RESID || a->epilogue == DWM_EPI_F32,
+                "dwm_b200_conv: E4M3 operands need epilogue DWM_EPI_RESID or DWM_EPI_F32, got %d", a->epilogue);
     DWM_REQUIRE(a->a_scale && a->w_scale, "dwm_b200_conv: E4M3 operands need a_scale [nb] and w_scale [c_out]");
     DWM_REQUIRE(a->c_in % 16 == 0, "dwm_b200_conv: E4M3 needs C_in %% 16 == 0 (16-byte TMA pitch); got %lld",
                 (long long)a->c_in);
     DWM_REQUIRE((reinterpret_cast<uintptr_t>(a->w_scale) & 7) == 0, "dwm_b200_conv: w_scale must be 8-byte aligned");
-    // the fp32-output epilogue never names its 16-bit type
+    // the fp32-output epilogues never name their 16-bit type
+    if (a->epilogue == DWM_EPI_F32) return conv_pick_bn_e4m3_f32(a, s);
     return conv_pick_bn<__nv_fp8_e4m3, __nv_bfloat16, DWM_EPI_RESID>(a, s);
   }
   set_last_error("dwm_b200_conv: dtype must be DWM_BF16, DWM_F16 or DWM_E4M3");

@@ -1,7 +1,7 @@
 // HBM-bound kernels of the CogVideoX temporal-VAE decoder (channels-last activations):
 // GroupNorm statistics, the fused SpatialNorm3D (GroupNorm * conv_y(zq) + conv_b(zq)) +
 // SiLU that writes the 16-bit, causally time-padded input of the next convolution (or, for
-// the FP8 UNet ResBlock convs, its E4M3 version with one scale per volume), and the
+// the FP8 UNet ResBlock and VAE ResNet convs, its E4M3 version with one scale per volume), and the
 // nearest-neighbour (space / space-time) upsampler.
 #include <algorithm>
 
@@ -145,14 +145,18 @@ struct SnParams {
   int stat_T;     // frames the GroupNorm sums cover (T, or the whole window of a frame shard)
   // HALO: frame-shard operand [nb, T + 2, H, W, C]; local frame 0 is also stored at frame
   // prev_T - 1 of prev_out, the last local frame at frame 0 of next_out (both [nb, *_T, H, W, C]);
-  // without a neighbour the own halo frame is stored as zero
+  // without a neighbour the own halo frame is stored as zero.
+  // SN_E4M3_TAIL (no HALO): next_out is the 16-bit [nb, 2, H, W, C] causal-conv cache of the
+  // next chunk, the operand's last two frames; prev_out the cache this call's operand starts with
+  // (NULL: a first chunk, whose leading frames replicate frame out_t0)
   void* prev_out = nullptr; int prev_T = 0;
   void* next_out = nullptr; int next_T = 0;
 };
 
 // What a spatialnorm_kernel pass does with each normalised float4: store it as 16 bit, only
-// fold it into the volume's amax, or store it as E4M3 with the volume's inverse scale.
-enum { SN_STORE16 = 0, SN_AMAX = 1, SN_E4M3 = 2 };
+// fold it into the volume's amax, or store it as E4M3 with the volume's inverse scale
+// (SN_E4M3_TAIL: and the operand's last two frames once more as T into next_out).
+enum { SN_STORE16 = 0, SN_AMAX = 1, SN_E4M3 = 2, SN_E4M3_TAIL = 3 };
 
 // grid = (chunks, nb): a block works on one chunk (16 float4 per thread) of ONE image, so the (mean, rstd) of its
 // G groups are finalised once per block from the fp64 sums (first G threads, shared memory)
@@ -199,7 +203,7 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
   // whole warps (C/4 = 80 gives 240 threads), hence no warp shuffles.
   float amax = 0.f;
   float inv = 0.f;
-  if constexpr (MODE == SN_E4M3) inv = e4m3_inv(__uint_as_float(reinterpret_cast<const uint32_t*>(p.scale)[n]));
+  if constexpr (MODE == SN_E4M3 || MODE == SN_E4M3_TAIL) inv = e4m3_inv(__uint_as_float(reinterpret_cast<const uint32_t*>(p.scale)[n]));
   auto store = [&](void* base, long long o, const float4& v) {
     if constexpr (MODE == SN_STORE16) {
       uint2 pk; pk.x = Cvt<T>::pack2(v.x, v.y); pk.y = Cvt<T>::pack2(v.z, v.w);
@@ -220,6 +224,17 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
       amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
     } else {
       store(p.out, o, v);
+      if constexpr (MODE == SN_E4M3_TAIL) {
+        // operand frame out_t0 + t is tail frame tt; with T = 1 and no previous tail, tail frame
+        // 0 is its replica
+        const int tt = t + 2 - p.T;
+        if (tt >= 0) {
+          uint2 pk; pk.x = Cvt<T>::pack2(v.x, v.y); pk.y = Cvt<T>::pack2(v.z, v.w);
+          const long long ot = o + (static_cast<long long>(n) * (2 - p.out_T) - p.out_t0 - t + tt) * frame4;
+          reinterpret_cast<uint2*>(p.next_out)[ot] = pk;
+          if (p.T == 1 && !p.prev_out) reinterpret_cast<uint2*>(p.next_out)[ot - frame4] = pk;
+        }
+      }
       if constexpr (HALO) {
         // o = ((n * out_T + out_t0 + t) * H*W + pixel) * vec + c4; re-based onto a neighbour's
         // frame by whole frames
@@ -348,6 +363,39 @@ __global__ void __launch_bounds__(1024) spatialnorm_kernel(const SnParams p, con
 __global__ void e4m3_amax_to_scale_kernel(const float* amax, float* scale, int nb) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n < nb) scale[n] = e4m3_scale(__uint_as_float(reinterpret_cast<const uint32_t*>(amax)[n]));
+}
+
+// The previous chunk's 16-bit causal-conv cache tail [nb, 2, H, W, C] (frame4 float4 groups per
+// frame) as frames out_t0 - 2, out_t0 - 1 of this chunk's E4M3 operand, under the chunk's volume
+// scale.  AMAX: folds max |tail| into the amax bits of each volume.  Else: quantizes the tail
+// with that amax and, when next_tail is given (T = 1: the new tail is tail frame 1 and the new
+// frame), stores tail frame 1 as next_tail's frame 0; tail and next_tail may be one buffer.
+template <typename T, bool AMAX>
+__global__ void __launch_bounds__(256) sn_tail_kernel(const void* tail, long long frame4, float* amax, void* out,
+                                                      int out_T, int out_t0, void* next_tail) {
+  const int n = blockIdx.y;
+  const uint2* src = reinterpret_cast<const uint2*>(tail) + static_cast<long long>(n) * 2 * frame4;
+  float inv = 0.f, a = 0.f;
+  if constexpr (!AMAX) inv = e4m3_inv(__uint_as_float(reinterpret_cast<const uint32_t*>(amax)[n]));
+  uint32_t* dst = reinterpret_cast<uint32_t*>(out) + (static_cast<long long>(n) * out_T + out_t0 - 2) * frame4;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < frame4;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const uint2 u[2] = {src[i], src[frame4 + i]};
+#pragma unroll
+    for (int f = 0; f < 2; ++f) {
+      const float2 lo = Cvt<T>::unpack2(u[f].x), hi = Cvt<T>::unpack2(u[f].y);
+      if constexpr (AMAX) a = fmaxf(a, fmaxf(fmaxf(fabsf(lo.x), fabsf(lo.y)), fmaxf(fabsf(hi.x), fabsf(hi.y))));
+      else dst[f * frame4 + i] = e4m3x4(lo.x, lo.y, hi.x, hi.y, inv);
+    }
+    if constexpr (!AMAX) {
+      if (next_tail) reinterpret_cast<uint2*>(next_tail)[static_cast<long long>(n) * 2 * frame4 + i] = u[1];
+    }
+  }
+  if constexpr (AMAX) {
+    // non-negative floats: the integer order of the bits is the float order
+    const unsigned int m = __reduce_max_sync(0xffffffffu, __float_as_uint(a));
+    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned int*>(amax) + n, m);
+  }
 }
 
 // ---- nearest upsample x2 in space, optionally in time (CogVideoXUpsample3D rules) ----
@@ -487,6 +535,62 @@ extern "C" int dwm_b200_groupnorm_silu_e4m3(const float* x, int64_t nb, int64_t 
   DWM_CHECK_CUDA(cudaMemsetAsync(out_scale, 0, sizeof(float) * nb, s));
   spatialnorm_kernel<__nv_fp8_e4m3, SN_AMAX><<<grid, threads, 0, s>>>(p, chunk);
   spatialnorm_kernel<__nv_fp8_e4m3, SN_E4M3><<<grid, threads, 0, s>>>(p, chunk);
+  e4m3_amax_to_scale_kernel<<<static_cast<unsigned>((nb + 127) / 128), 128, 0, s>>>(out_scale, out_scale, (int)nb);
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dwm_b200_spatialnorm_silu_e4m3(const float* x, int64_t nb, int64_t T, int64_t H, int64_t W, int C,
+                                              int groups, const double* sums, float eps, const float* gamma,
+                                              const float* beta, const float* zy, const float* zb, int Tz, int hz,
+                                              int wz, int apply_silu, void* out, int64_t out_T, int64_t out_t0,
+                                              float* out_scale, const void* tail_in, void* tail_out, int tail_dtype,
+                                              dwm_stream_t stream) {
+  DWM_REQUIRE(x && sums && gamma && beta && out && out_scale, "dwm_b200_spatialnorm_silu_e4m3: null pointer");
+  DWM_REQUIRE(nb > 0 && T > 0 && H > 0 && W > 0 && nb <= 65535, "dwm_b200_spatialnorm_silu_e4m3: bad shape");
+  DWM_REQUIRE(C % 16 == 0 && groups > 0 && C % groups == 0 && groups <= 64,
+              "dwm_b200_spatialnorm_silu_e4m3: need C %% 16 == 0, C %% groups == 0, groups <= 64 (got C=%d, groups=%d)",
+              C, groups);
+  DWM_REQUIRE((zy == nullptr) == (zb == nullptr), "dwm_b200_spatialnorm_silu_e4m3: zy and zb go together");
+  DWM_REQUIRE(out_t0 >= 0 && out_t0 + T <= out_T, "dwm_b200_spatialnorm_silu_e4m3: frame window outside out buffer");
+  DWM_REQUIRE(!tail_in || out_t0 >= 2, "dwm_b200_spatialnorm_silu_e4m3: tail_in needs out_t0 >= 2");
+  DWM_REQUIRE(!(tail_in || tail_out) || tail_dtype == DWM_BF16 || tail_dtype == DWM_F16,
+              "dwm_b200_spatialnorm_silu_e4m3: tail_dtype must be DWM_BF16 or DWM_F16");
+  DWM_REQUIRE(!gn_align_check(x, sums, gamma, beta, zy, zb) && is_aligned(out, 4) && is_aligned(tail_in, 8) &&
+                  is_aligned(tail_out, 8),
+              "dwm_b200_spatialnorm_silu_e4m3: x, gamma, beta, zy, zb must be 16-byte, sums, tail_in, tail_out "
+              "8-byte and out 4-byte aligned");
+  SnParams p;
+  p.x = x; p.nb = (int)nb; p.T = (int)T; p.H = (int)H; p.W = (int)W; p.C = C; p.G = groups;
+  p.sums = sums; p.eps = eps; p.gamma = gamma; p.beta = beta; p.zy = zy; p.zb = zb;
+  p.Tz = Tz; p.hz = hz; p.wz = wz; p.silu = apply_silu; p.out = out; p.out_T = (int)out_T; p.out_t0 = (int)out_t0;
+  p.scale = out_scale; p.stat_T = (int)T;
+  p.prev_out = const_cast<void*>(tail_in); p.next_out = tail_out;
+  const long long per_img = T * H * W * (C / 4);
+  const int vec = C / 4;
+  int threads = 256;
+  if (vec <= 1024) threads = vec <= 256 ? (256 / vec) * vec : vec;
+  const int chunk = threads * 16;
+  dim3 grid(static_cast<unsigned>((per_img + chunk - 1) / chunk), static_cast<unsigned>(nb));
+  const long long frame4 = H * W * (C / 4);
+  dim3 tgrid(static_cast<unsigned>(std::min<long long>((frame4 + 1023) / 1024, 2048)), static_cast<unsigned>(nb));
+  const bool bf = tail_dtype == DWM_BF16;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  DWM_CHECK_CUDA(cudaMemsetAsync(out_scale, 0, sizeof(float) * nb, s));
+  // amax over the cached tail and the new frames, then both quantized with the one volume scale
+  if (tail_in) {
+    if (bf) sn_tail_kernel<__nv_bfloat16, true><<<tgrid, 256, 0, s>>>(tail_in, frame4, out_scale, out, p.out_T, p.out_t0, nullptr);
+    else sn_tail_kernel<__half, true><<<tgrid, 256, 0, s>>>(tail_in, frame4, out_scale, out, p.out_T, p.out_t0, nullptr);
+  }
+  spatialnorm_kernel<__nv_fp8_e4m3, SN_AMAX><<<grid, threads, 0, s>>>(p, chunk);
+  if (tail_in) {
+    void* shift = T == 1 ? tail_out : nullptr;
+    if (bf) sn_tail_kernel<__nv_bfloat16, false><<<tgrid, 256, 0, s>>>(tail_in, frame4, out_scale, out, p.out_T, p.out_t0, shift);
+    else sn_tail_kernel<__half, false><<<tgrid, 256, 0, s>>>(tail_in, frame4, out_scale, out, p.out_T, p.out_t0, shift);
+  }
+  if (!tail_out) spatialnorm_kernel<__nv_fp8_e4m3, SN_E4M3><<<grid, threads, 0, s>>>(p, chunk);
+  else if (bf) spatialnorm_kernel<__nv_bfloat16, SN_E4M3_TAIL><<<grid, threads, 0, s>>>(p, chunk);
+  else spatialnorm_kernel<__half, SN_E4M3_TAIL><<<grid, threads, 0, s>>>(p, chunk);
   e4m3_amax_to_scale_kernel<<<static_cast<unsigned>((nb + 127) / 128), 128, 0, s>>>(out_scale, out_scale, (int)nb);
   DWM_CHECK_CUDA(cudaGetLastError());
   return 0;

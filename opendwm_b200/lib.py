@@ -132,6 +132,10 @@ SYMBOLS = {
     "dwm_b200_groupnorm_silu_e4m3": (ctypes.c_int, [
         _p, _i64, _i64, _i64, _i64, ctypes.c_int, ctypes.c_int, _p, ctypes.c_float,
         _p, _p, ctypes.c_int, _p, _i64, _i64, _p, _p]),
+    "dwm_b200_spatialnorm_silu_e4m3": (ctypes.c_int, [
+        _p, _i64, _i64, _i64, _i64, ctypes.c_int, ctypes.c_int, _p, ctypes.c_float,
+        _p, _p, _p, _p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _p,
+        _i64, _i64, _p, _p, _p, ctypes.c_int, _p]),
     "dwm_b200_groupnorm_silu_halo": (ctypes.c_int, [
         _p, _i64, _i64, _i64, _i64, ctypes.c_int, ctypes.c_int, _p, _i64, ctypes.c_float,
         _p, _p, ctypes.c_int, _p, _p, _i64, _p, _i64, ctypes.c_int, _p]),

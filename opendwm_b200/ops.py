@@ -491,7 +491,8 @@ def conv(x, weight, bias=None, *, kernel, epilogue=_l.EPI_F32, act=_l.ACT_NONE,
     """x: 16-bit channels-last [nb, tp, h, w, c_in]; weight: tap-major
     [kt*kh*kw, c_out, c_in]; returns [nb*(tp-kt+1)*h*w, c_out].
     FP8: x and weight float8_e4m3fn with a_scale fp32 [nb] (one per volume,
-    groupnorm_silu_e4m3) and w_scale fp32 [c_out] (pack_conv_weight_fp8); RESID only."""
+    groupnorm_silu_e4m3 / spatialnorm_silu_e4m3) and w_scale fp32 [c_out]
+    (pack_conv_weight_fp8); RESID, or F32 with c_out % 128 == 0."""
     if x.dim() != 5 or not x.is_contiguous() or not weight.is_contiguous():
         raise ValueError("conv: x must be contiguous [nb, tp, h, w, c]")
     if not x.is_cuda:
@@ -505,8 +506,10 @@ def conv(x, weight, bias=None, *, kernel, epilogue=_l.EPI_F32, act=_l.ACT_NONE,
     if fp8:
         if a_scale is None or w_scale is None:
             raise ValueError("conv: FP8 operands need a_scale and w_scale")
-        if epilogue != _l.EPI_RESID:
-            raise ValueError("conv: FP8 operands need the RESID epilogue")
+        if epilogue != _l.EPI_RESID and (epilogue != _l.EPI_F32 or c_out % 128):
+            raise ValueError("conv: FP8 operands need the RESID epilogue, or F32 with "
+                             "c_out % 128 == 0; got epilogue {} with c_out {}".format(
+                                 epilogue, c_out))
         for t, n, name in ((a_scale, nb, "a_scale"), (w_scale, c_out, "w_scale")):
             _f32(t, name)
             if t.dim() != 1 or t.numel() != n:
@@ -583,23 +586,69 @@ def spatialnorm_silu(x, sums, gamma, beta, out, *, groups, eps=1e-6, zy=None,
     if out.dim() != 5 or not out.is_contiguous() or out.shape[0] != nb or out.shape[2:] != x.shape[2:]:
         raise ValueError("out must be contiguous [nb, out_T, H, W, C]")
     _check_gn_operands(sums, gamma, beta, nb, C, groups)
-    Tz = hz = wz = 0
-    if (zy is None) != (zb is None):
-        raise ValueError("zy and zb go together")
-    if zy is not None:
-        for t, name in ((zy, "zy"), (zb, "zb")):
-            _f32(t, name)
-            if t.dim() != 5 or not t.is_contiguous() or t.shape[0] != nb or t.shape[4] != C:
-                raise ValueError("{} must be contiguous fp32 [nb, Tz, hz, wz, C]".format(name))
-        if zb.shape != zy.shape:
-            raise ValueError("zy and zb shapes differ")
-        Tz, hz, wz = zy.shape[1:4]
+    Tz, hz, wz = _spatial_mod(zy, zb, nb, C)
     _l.check(_l.load().dwm_b200_spatialnorm_silu(
         x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), eps,
         _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(),
         _ptr(zy), _ptr(zb), Tz, hz, wz, int(silu), out.data_ptr(), out.shape[1],
         out_t0, _dt(out), _stream()), "dwm_b200_spatialnorm_silu")
     return out
+
+
+def _spatial_mod(zy, zb, nb, C):
+    """(Tz, hz, wz) of the SpatialNorm3D modulation zy / zb fp32 [nb, Tz, hz, wz, C] (zeros
+    without one)."""
+    if (zy is None) != (zb is None):
+        raise ValueError("zy and zb go together")
+    if zy is None:
+        return 0, 0, 0
+    for t, name in ((zy, "zy"), (zb, "zb")):
+        _f32(t, name)
+        if t.dim() != 5 or not t.is_contiguous() or t.shape[0] != nb or t.shape[4] != C:
+            raise ValueError("{} must be contiguous fp32 [nb, Tz, hz, wz, C]".format(name))
+    if zb.shape != zy.shape:
+        raise ValueError("zy and zb shapes differ")
+    return tuple(zy.shape[1:4])
+
+
+def spatialnorm_silu_e4m3(x, sums, gamma, beta, out, scale, *, groups, eps=1e-6, zy=None,
+                          zb=None, out_t0=0, silu=True, tail_in=None, tail_out=None):
+    """SpatialNorm3D(+SiLU) of x fp32 [nb,T,H,W,C] (zy / zb as in spatialnorm_silu) into E4M3
+    out [nb,out_T,H,W,C] (frames [out_t0, out_t0+T)) with one fp32 scale per volume in
+    scale [nb].  tail_in (16-bit [nb,2,H,W,C]): the previous chunk's causal-conv cache, covered
+    by the volume's amax and quantized into frames out_t0-2, out_t0-1.  tail_out (same
+    layout and dtype, may be tail_in): receives the operand's last two frames in 16 bit."""
+    _f32(x, "x")
+    if x.dim() != 5 or not x.is_contiguous():
+        raise ValueError("x must be contiguous [nb, T, H, W, C]")
+    nb, T, H, W, C = x.shape
+    for t, name in ((out, "out"), (scale, "scale"), (sums, "sums"), (gamma, "gamma"),
+                    (beta, "beta"), (zy, "zy"), (zb, "zb"), (tail_in, "tail_in"),
+                    (tail_out, "tail_out")):
+        if t is not None and t.device != x.device:
+            raise RuntimeError("spatialnorm_silu_e4m3: {} is on {}, x on {} (every operand on "
+                               "x's GPU; no CPU fallback)".format(name, t.device, x.device))
+    if out.dtype != FP8 or out.dim() != 5 or not out.is_contiguous() or \
+            out.shape[0] != nb or out.shape[2:] != x.shape[2:]:
+        raise ValueError("out must be contiguous float8_e4m3fn [nb, out_T, H, W, C]")
+    _f32(scale, "scale")
+    if scale.numel() != nb or not scale.is_contiguous():
+        raise ValueError("scale must be fp32 [nb]")
+    _check_gn_operands(sums, gamma, beta, nb, C, groups)
+    Tz, hz, wz = _spatial_mod(zy, zb, nb, C)
+    tails = [t for t in (tail_in, tail_out) if t is not None]
+    for t in tails:
+        if t.dtype != tails[0].dtype or t.dim() != 5 or not t.is_contiguous() or \
+                tuple(t.shape) != (nb, 2, H, W, C):
+            raise ValueError("tail_in / tail_out must be contiguous 16-bit [nb, 2, H, W, C] of "
+                             "one dtype")
+    _l.check(_l.load().dwm_b200_spatialnorm_silu_e4m3(
+        x.data_ptr(), nb, T, H, W, C, groups, sums.data_ptr(), eps,
+        _f32(gamma, "gamma").data_ptr(), _f32(beta, "beta").data_ptr(),
+        _ptr(zy), _ptr(zb), Tz, hz, wz, int(silu), out.data_ptr(), out.shape[1], out_t0,
+        scale.data_ptr(), _ptr(tail_in), _ptr(tail_out), _dt(tails[0]) if tails else 0,
+        _stream()), "dwm_b200_spatialnorm_silu_e4m3")
+    return out, scale
 
 
 def groupnorm_silu_e4m3(x, sums, gamma, beta, out, scale, *, groups, eps=1e-6, out_t0=0,

@@ -18,6 +18,11 @@ mid-block attention is computed per image as S = Q K^T (GEMM, fp32 out), a row s
 kernel, and O = P V against V^T, which the V projection produces directly
 (V^T = W_v X^T); the V bias commutes with the softmax average and is folded into the
 output-projection bias.
+
+gemm_dtype=torch.float8_e4m3fn runs conv1 / conv2 of every decoder ResNet block (mid and up
+blocks) in E4M3, with one activation scale per image and one weight scale per output channel;
+conv_in / conv_out, the upsampler convs, the shortcuts, the mid-block attention and the encoder
+stay 16-bit.
 """
 import json
 import math
@@ -28,7 +33,8 @@ import torch
 from opendwm_b200 import lib as _lib
 from opendwm_b200 import ops as _ops
 
-from .packing import Linear, conv, fp32, gemm, pack_conv, pack_linear, pack_norm
+from .packing import (
+    FP8, Linear, Operand, conv, fp32, gemm, pack_conv, pack_linear, pack_norm)
 
 
 class _Cfg(dict):
@@ -60,9 +66,9 @@ def _attention(channels, groups):
     return m
 
 
-def _pack_resnet(m, dt, dev):
-    p = dict(n1=pack_norm(m.norm1), c1=pack_conv(m.conv1, dt, dev), n2=pack_norm(m.norm2),
-             c2=pack_conv(m.conv2, dt, dev))
+def _pack_resnet(m, dt, dev, fp8=False):
+    p = dict(n1=pack_norm(m.norm1), c1=pack_conv(m.conv1, dt, dev, fp8), n2=pack_norm(m.norm2),
+             c2=pack_conv(m.conv2, dt, dev, fp8))
     if hasattr(m, "conv_shortcut"):
         p["sc"] = pack_linear(m.conv_shortcut.weight, m.conv_shortcut.bias, dt, dev)
     return p
@@ -107,8 +113,14 @@ class AutoencoderKL(torch.nn.Module):
                  act_fn="silu", latent_channels=4, norm_num_groups=32, sample_size=32,
                  scaling_factor=0.18215, shift_factor=None, force_upcast=True,
                  use_quant_conv=True, use_post_quant_conv=True,
-                 mid_block_add_attention=True, compute_dtype=torch.bfloat16, **unused):
+                 mid_block_add_attention=True, compute_dtype=torch.bfloat16, gemm_dtype=None,
+                 **unused):
+        """gemm_dtype=torch.float8_e4m3fn runs the decoder ResNet convolutions in E4M3 (see
+        the module docstring); None keeps every convolution 16-bit."""
         super().__init__()
+        if gemm_dtype not in (None, torch.float8_e4m3fn):
+            raise ValueError(
+                "gemm_dtype must be None or torch.float8_e4m3fn, got {!r}".format(gemm_dtype))
         if act_fn != "silu":
             raise NotImplementedError("AutoencoderKL act_fn {}".format(act_fn))
         boc = tuple(block_out_channels)
@@ -121,6 +133,8 @@ class AutoencoderKL(torch.nn.Module):
             mid_block_add_attention=mid_block_add_attention,
             down_block_types=tuple(down_block_types or ("DownEncoderBlock2D",) * len(boc)))
         self.compute_dtype = compute_dtype
+        self.gemm_dtype = gemm_dtype
+        self._ws8 = {}
         g = norm_num_groups
         rev = list(reversed(boc))
         d = _P()
@@ -205,6 +219,7 @@ class AutoencoderKL(torch.nn.Module):
 
     def _apply(self, fn, *a, **k):
         self._pk = self._pk_enc = None
+        self._ws8 = {}
         return super()._apply(fn, *a, **k)
 
     def load_state_dict(self, state_dict, strict=True, assign=False):
@@ -212,6 +227,7 @@ class AutoencoderKL(torch.nn.Module):
         keys keep their initial values); the pre-0.20 attention names (query/key/value/
         proj_attn) are accepted like diffusers' `_convert_deprecated_attention_blocks` does."""
         self._pk = self._pk_enc = None
+        self._ws8 = {}
         ren = {"query": "to_q", "key": "to_k", "value": "to_v", "proj_attn": "to_out.0"}
         sd = {}
         for k, v in state_dict.items():
@@ -253,13 +269,14 @@ class AutoencoderKL(torch.nn.Module):
             pk = dict(pq=Linear(w, b), conv_in=pack_conv(d.conv_in, dt, dev, pad_in=cq))
         else:
             pk = dict(conv_in=pack_conv(d.conv_in, dt, dev, pad_in=cp))
-        pk["mid"] = [_pack_resnet(r, dt, dev) for r in d.mid_block.resnets]
+        fp8 = self.gemm_dtype is not None
+        pk["mid"] = [_pack_resnet(r, dt, dev, fp8) for r in d.mid_block.resnets]
         pk["attn"] = None
         if len(d.mid_block.attentions):
             pk["attn"] = _pack_attention(d.mid_block.attentions[0], dt, dev)
         pk["ups"] = []
         for blk in d.up_blocks:
-            b = dict(res=[_pack_resnet(r, dt, dev) for r in blk.resnets])
+            b = dict(res=[_pack_resnet(r, dt, dev, fp8) for r in blk.resnets])
             if hasattr(blk, "upsamplers"):
                 b["up"] = pack_conv(blk.upsamplers[0].conv, dt, dev)
             pk["ups"].append(b)
@@ -281,10 +298,28 @@ class AutoencoderKL(torch.nn.Module):
         _ops.spatialnorm_silu(h5, sums, p[0], p[1], out, groups=groups, eps=p[2], silu=silu)
         return out
 
+    def _norm_silu_operand(self, h, shape, g, c):
+        """GroupNorm + SiLU of fp32 rows as the operand of conv c: 16-bit, or for an E4M3 c
+        E4M3 with one scale per image (in a workspace kept across calls of one geometry)."""
+        if c.scale is None:
+            return self._norm(h, shape, g, True)
+        nb, H, W = shape
+        C = h.shape[1]
+        h5 = h.view(nb, 1, H, W, C)
+        groups = self.config.norm_num_groups
+        sums = _ops.groupnorm_stats(h5, groups)
+        ws = self._ws8.get((nb, H, W, C))
+        if ws is None:
+            ws = self._ws8[nb, H, W, C] = (
+                torch.empty(nb, 1, H, W, C, device=h.device, dtype=FP8),
+                torch.empty(nb, device=h.device, dtype=torch.float32))
+        return Operand(*_ops.groupnorm_silu_e4m3(h5, sums, g[0], g[1], *ws, groups=groups,
+                                                 eps=g[2], silu=True))
+
     def _resnet(self, h, shape, p):
-        a = self._norm(h, shape, p["n1"], True)
+        a = self._norm_silu_operand(h, shape, p["n1"], p["c1"])
         h1 = conv(a, p["c1"], kernel=(1, 3, 3), epilogue=_lib.EPI_F32)
-        b = self._norm(h1, shape, p["n2"], True)
+        b = self._norm_silu_operand(h1, shape, p["n2"], p["c2"])
         if "sc" in p:
             h16 = torch.empty(h.shape, device=h.device, dtype=self.compute_dtype)
             _ops.act_cast(h, h16)

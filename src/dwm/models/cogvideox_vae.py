@@ -19,6 +19,14 @@ causal temporal padding = two cached frames kept in front of each conv input buf
 SpatialNorm3D (GroupNorm * conv_y(zq) + conv_b(zq)) + SiLU is one fused pass that emits
 the next convolution's 16-bit input; conv_y / conv_b / conv_shortcut (1x1x1) run on the
 wgmma GEMM at latent resolution; residual adds are conv epilogues.
+
+gemm_dtype=torch.float8_e4m3fn runs conv1 / conv2 of every decoder ResNet block (mid and up
+blocks) in E4M3: one activation scale per volume (one (b v) item of one chunk, cached frames
+included), one weight scale per output channel.  The causal-conv cache stays 16-bit: the two
+cached frames of the previous chunk are folded into this chunk's amax and quantized with its
+scale (an E4M3 tail would carry the previous chunk's scale, which does not factor out of the
+sum over taps).  conv_in / conv_out, the upsampler convs, the shortcuts, conv_y / conv_b and
+the encoder stay 16-bit.
 """
 import json
 import math
@@ -29,7 +37,7 @@ import torch
 from opendwm_b200 import lib as _lib
 from opendwm_b200 import ops as _ops
 
-from .packing import conv, gemm, pack_conv, pack_linear, pack_norm
+from .packing import FP8, Operand, conv, gemm, pack_conv, pack_linear, pack_norm
 
 
 class _Cfg(dict):
@@ -91,8 +99,13 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
                  layers_per_block=3, norm_num_groups=32,
                  temporal_compression_ratio=4, scaling_factor=1.15258426,
                  shift_factor=None, compute_dtype=torch.bfloat16, with_encoder=False,
-                 **unused):
+                 gemm_dtype=None, **unused):
+        """gemm_dtype=torch.float8_e4m3fn runs the decoder ResNet convolutions in E4M3 (see
+        the module docstring); None keeps every convolution 16-bit."""
         super().__init__()
+        if gemm_dtype not in (None, torch.float8_e4m3fn):
+            raise ValueError(
+                "gemm_dtype must be None or torch.float8_e4m3fn, got {!r}".format(gemm_dtype))
         self.config = _Cfg(
             in_channels=in_channels, out_channels=out_channels,
             block_out_channels=tuple(block_out_channels),
@@ -102,6 +115,8 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
             scaling_factor=scaling_factor, shift_factor=shift_factor,
             down_block_types=("CogVideoXDownBlock3D",) * len(block_out_channels))
         self.compute_dtype = compute_dtype
+        self.gemm_dtype = gemm_dtype
+        self._ws8 = {}
         self.num_latent_frames_batch_size = 2
         g = norm_num_groups
         rev = list(reversed(block_out_channels))
@@ -195,10 +210,12 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
 
     def _apply(self, fn, *a, **k):
         self._pk = self._pk_enc = None
+        self._ws8 = {}
         return super()._apply(fn, *a, **k)
 
     def load_state_dict(self, state_dict, strict=True, assign=False):
         self._pk = self._pk_enc = None
+        self._ws8 = {}
         return super().load_state_dict(state_dict, strict=strict, assign=assign)
 
     # -- weight packing --------------------------------------------------------------------
@@ -209,10 +226,13 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
             raise RuntimeError("AutoencoderKLCogVideoX.decode runs on CUDA (sm_90a) "
                                "only; there is no CPU fallback.")
         dt = self.compute_dtype
+        fp8 = self.gemm_dtype is not None
 
         def res(m):
-            p = dict(n1=_pack_spatial_norm(m.norm1, dt, dev), c1=pack_conv(m.conv1.conv, dt, dev),
-                     n2=_pack_spatial_norm(m.norm2, dt, dev), c2=pack_conv(m.conv2.conv, dt, dev))
+            p = dict(n1=_pack_spatial_norm(m.norm1, dt, dev),
+                     c1=pack_conv(m.conv1.conv, dt, dev, fp8),
+                     n2=_pack_spatial_norm(m.norm2, dt, dev),
+                     c2=pack_conv(m.conv2.conv, dt, dev, fp8))
             if hasattr(m, "conv_shortcut"):
                 p["sc"] = pack_linear(m.conv_shortcut.weight, m.conv_shortcut.bias, dt, dev)
             return p
@@ -234,7 +254,10 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
     # -- building blocks ---------------------------------------------------------------------
     def _causal_conv(self, name, x_pad, c, cache, new_cache, **kw):
         """x_pad: 16-bit [nb, T+2, H, W, C] whose frames [2:] are filled; the two leading
-        frames become the cached tail of the previous chunk or replicas of frame 0."""
+        frames become the cached tail of the previous chunk or replicas of frame 0.  An E4M3
+        Operand of `_norm_operand` has its cache frames already in place."""
+        if isinstance(x_pad, Operand):
+            return conv(x_pad, c, kernel=(3, 3, 3), **kw)
         prev = cache.get(name)
         if prev is not None:
             x_pad[:, :2].copy_(prev)
@@ -246,25 +269,76 @@ class AutoencoderKLCogVideoX(torch.nn.Module):
         new_cache[name] = x_pad[:, -2:]
         return conv(x_pad, c, kernel=(3, 3, 3), **kw)
 
-    def _norm_act(self, h, shape, p, zq16, zshape, groups):
-        """SpatialNorm3D + SiLU of fp32 `h` [rows, C] -> 16-bit time-padded conv input."""
+    def _norm_operands(self, h, shape, p, zq16, zshape, groups):
+        """(h as [nb, T, H, W, C], its GroupNorm sums, zy, zb) of a SpatialNorm3D."""
         nb, T, H, W = shape
         C = h.shape[1]
         h5 = h.view(nb, T, H, W, C)
         sums = _ops.groupnorm_stats(h5, groups)
         zy = gemm(zq16, p["y"], epilogue=_lib.EPI_F32).view(*zshape, C)
         zb = gemm(zq16, p["b"], epilogue=_lib.EPI_F32).view(*zshape, C)
+        return h5, sums, zy, zb
+
+    def _norm_act(self, h, shape, p, zq16, zshape, groups):
+        """SpatialNorm3D + SiLU of fp32 `h` [rows, C] -> 16-bit time-padded conv input."""
+        h5, sums, zy, zb = self._norm_operands(h, shape, p, zq16, zshape, groups)
+        nb, T, H, W, C = h5.shape
         out = torch.empty(nb, T + 2, H, W, C, device=h.device, dtype=self.compute_dtype)
         g = p["norm"]
         _ops.spatialnorm_silu(h5, sums, g[0], g[1], out, groups=groups,
                               eps=g[2], zy=zy, zb=zb, out_t0=2, silu=True)
         return out
 
+    def _buf8(self, key, shape, dtype):
+        """Workspace kept across calls of one geometry: each FP8 conv's 16-bit cache tail
+        (2 frames per volume) and the volume scales."""
+        k = (key, tuple(shape), dtype)
+        if k not in self._ws8:
+            self._ws8[k] = torch.empty(shape, device=self.decoder.conv_in.conv.weight.device,
+                                       dtype=dtype)
+        return self._ws8[k]
+
+    def _operand8(self, shape):
+        """The E4M3 operand of an FP8 conv: a view of ONE buffer that every FP8 conv shares
+        (each conv reads it before the next SpatialNorm writes it, in stream order), grown to
+        the largest operand seen and kept across calls."""
+        n = math.prod(shape)
+        buf = self._ws8.get("x8")
+        if buf is None or buf.numel() < n:
+            buf = self._ws8["x8"] = torch.empty(
+                n, device=self.decoder.conv_in.conv.weight.device, dtype=FP8)
+        return buf[:n].view(shape)
+
+    def _norm_operand(self, name, h, shape, p, c, zq16, zshape, groups, cache, new_cache):
+        """SpatialNorm3D + SiLU of fp32 `h` as the operand of the causal conv c (a ResNet conv1 /
+        conv2): 16-bit (`_causal_conv` fills its cache frames), or for an E4M3 c an E4M3
+        Operand whose volume scale covers the 16-bit cache tail of the previous chunk, with the
+        operand's last two frames kept in 16 bit as the next tail."""
+        if c.scale is None:
+            return self._norm_act(h, shape, p, zq16, zshape, groups)
+        h5, sums, zy, zb = self._norm_operands(h, shape, p, zq16, zshape, groups)
+        nb, T, H, W, C = h5.shape
+        x8 = self._operand8((nb, T + 2, H, W, C))
+        scale = self._buf8("x8_scale", (nb,), torch.float32)
+        prev = cache.get(name)
+        tail = self._buf8(name, (nb, 2, H, W, C), self.compute_dtype)
+        g = p["norm"]
+        _ops.spatialnorm_silu_e4m3(h5, sums, g[0], g[1], x8, scale, groups=groups, eps=g[2],
+                                   zy=zy, zb=zb, out_t0=2, silu=True, tail_in=prev,
+                                   tail_out=tail)
+        if prev is None:      # replicas of frame 0: its bytes, under the same scale
+            b = x8.view(torch.uint8)
+            b[:, :2].copy_(b[:, 2:3].expand(-1, 2, -1, -1, -1))
+        new_cache[name] = tail
+        return Operand(x8, scale)
+
     def _resnet(self, name, h, shape, p, zq16, zshape, groups, cache, new_cache):
-        a = self._norm_act(h, shape, p["n1"], zq16, zshape, groups)
+        a = self._norm_operand(name + ".conv1", h, shape, p["n1"], p["c1"], zq16, zshape,
+                               groups, cache, new_cache)
         h1 = self._causal_conv(name + ".conv1", a, p["c1"], cache, new_cache,
                                epilogue=_lib.EPI_F32)
-        b = self._norm_act(h1, shape, p["n2"], zq16, zshape, groups)
+        b = self._norm_operand(name + ".conv2", h1, shape, p["n2"], p["c2"], zq16, zshape,
+                               groups, cache, new_cache)
         if "sc" in p:
             h16 = torch.empty(h.shape, device=h.device, dtype=self.compute_dtype)
             _ops.act_cast(h, h16)

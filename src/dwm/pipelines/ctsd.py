@@ -30,6 +30,15 @@ from dwm.schedulers import temporal_independent as _ti
 from opendwm_b200 import ops as _ops
 
 
+def load_vae(vae_type, vae_path, common_config):
+    """vae_type.from_pretrained(vae_path, subfolder="vae"), with common_config["vae_gemm_dtype"]
+    (a dtype, or its {"_class_name": "get_class", "class_name": ...} config) as the opt-in
+    gemm_dtype of the decoder ResNet convolutions."""
+    gemm_dtype = dwm.common.create_instance_from_config(common_config.get("vae_gemm_dtype"))
+    kw = {} if gemm_dtype is None else {"gemm_dtype": gemm_dtype}
+    return vae_type.from_pretrained(vae_path, subfolder="vae", **kw)
+
+
 class CrossviewTemporalSD:
 
     @staticmethod
@@ -270,7 +279,7 @@ class CrossviewTemporalSD:
                 from dwm.models.autoencoder_kl import AutoencoderKL as vae_type
             else:
                 raise Exception("Unsupported VAE type {}.".format(vae_name))
-            self.vae = vae_type.from_pretrained(vae_path, subfolder="vae").to(self.device)
+            self.vae = load_vae(vae_type, vae_path, common_config).to(self.device)
         if self.vae is not None and \
                 type(self.vae).__name__ == "AutoencoderKLCogVideoX":
             self.is_temporal_vae = True

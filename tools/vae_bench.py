@@ -20,7 +20,7 @@ def decoder_flops(vae, frames, h, w):
     rev = list(reversed(cfgv.block_out_channels))
     total = 0.0
     fb, rem = 2, frames % 2
-    chunks = [(0, fb + rem)] + [(fb * i + rem, fb * (i + 1) + rem) for i in range(1, frames // fb)]
+    chunks = [(0, min(frames, fb + rem))] + [(fb * i + rem, fb * (i + 1) + rem) for i in range(1, frames // fb)]
     for a, b in chunks:
         T, H, W = b - a, h, w
         total += 2 * T * H * W * 27 * cfgv.latent_channels * rev[0]
