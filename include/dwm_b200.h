@@ -37,7 +37,10 @@ extern "C" {
 typedef void* dwm_stream_t; /* cudaStream_t */
 
 enum dwm_dtype { DWM_BF16 = 0, DWM_F16 = 1, DWM_F32 = 2, DWM_E4M3 = 3 };
-enum dwm_act { DWM_ACT_NONE = 0, DWM_ACT_GELU_TANH = 1, DWM_ACT_GELU_ERF = 2, DWM_ACT_SILU = 3, DWM_ACT_RELU = 4 };
+/* DWM_ACT_QUICK_GELU: x * sigmoid(1.702 x) (CLIP-L's quick_gelu); DWM_EPI_STORE with
+ * 16-bit operands only. */
+enum dwm_act { DWM_ACT_NONE = 0, DWM_ACT_GELU_TANH = 1, DWM_ACT_GELU_ERF = 2, DWM_ACT_SILU = 3, DWM_ACT_RELU = 4,
+               DWM_ACT_QUICK_GELU = 5 };
 
 /* Epilogues of dwm_b200_linear (all fused into the wgmma GEMM kernel). */
 enum dwm_epilogue {
@@ -59,7 +62,11 @@ enum dwm_epilogue {
    * (JointTransformerBlock gated residuals; AlphaBlender crossview_temporal.py:53-72) */
   DWM_EPI_RESID = 3,
   /* out32[m, n] = act(acc + bias[n]) */
-  DWM_EPI_F32 = 4
+  DWM_EPI_F32 = 4,
+  /* gated tanh-GELU (T5 v1.1 DenseGatedActDense, feed_forward_proj="gated-gelu"):
+   * the weight packed as for DWM_EPI_GEGLU with value rows wi_1 and gate rows wi_0;
+   * out16[m, j] = (acc_v + b_v) * gelu_tanh(acc_g + b_g), out width N/2.  16-bit operands. */
+  DWM_EPI_GEGLU_TANH = 5
 };
 
 typedef struct dwm_linear_args {
@@ -208,6 +215,15 @@ typedef struct dwm_attention_args {
 
 int dwm_b200_attention(const dwm_attention_args* args, dwm_stream_t stream);
 
+/* Text-encoder attention (CLIP / T5 self-attention over 77-token prompts): dwm_b200_attention
+ * with causal != 0 masking key j > query i (CLIP), or with bias (fp32 [heads, seq, seq], shared
+ * by every group) added to the scaled scores before the softmax (T5's relative-position bias);
+ * one of the two.  Contiguous sequences only (group_dims[1] = group_dims[2] = 1, inner = seq =
+ * group_strides[0], unit strides, no mask / kv / split), any seq >= 1.  They run on the wgmma
+ * kernel whatever "attn_tc" says; a call it cannot serve returns < 0. */
+int dwm_b200_attention_text(const dwm_attention_args* args, int causal, const float* bias,
+                            dwm_stream_t stream);
+
 /* ---- row ops ---------------------------------------------------------------------- */
 /* LayerNorm over the last dim of an fp32 residual stream, emitting the 16-bit GEMM operand.
  *   t = x[m] (+ add_item[m / rows_per_item]) (+ add_full[m]);  if sum_out: sum_out[m] = t
@@ -248,6 +264,19 @@ typedef struct dwm_layernorm_args {
 } dwm_layernorm_args;
 
 int dwm_b200_layernorm(const dwm_layernorm_args* args, dwm_stream_t stream);
+
+/* RMSNorm of an fp32 stream (T5LayerNorm): out[m] = weight * x[m] * rsqrt(mean(x[m]^2) + eps),
+ * statistics in fp32, out of dtype DWM_BF16 / DWM_F16 (the GEMM operand) or DWM_F32.  D and the
+ * pitches ldx / ldo are multiples of 4; x, weight 16-byte and out 8-byte (fp32: 16-byte) aligned. */
+int dwm_b200_rmsnorm(const float* x, int64_t M, int64_t D, int64_t ldx, const float* weight, float eps,
+                     void* out, int64_t ldo, int dtype, dwm_stream_t stream);
+
+/* Token (and absolute position) embedding gather into the fp32 residual stream of a text encoder:
+ *   out[m, :] = tok[ids[m], :] (+ pos[m % seq, :])
+ * ids int64 [M] (each < vocab; a bad id traps), tok fp32 [vocab, D], pos fp32 [>= seq, D] or NULL,
+ * out fp32 [M, ldo].  One fp32 add: bit-exact against torch's embedding + add. */
+int dwm_b200_embed(const int64_t* ids, int64_t M, int64_t seq, const float* tok, int64_t vocab,
+                   const float* pos, int64_t D, float* out, int64_t ldo, dwm_stream_t stream);
 
 /* Row-wise E4M3 quantization of a GEMM operand: x [M, K] (dtype DWM_BF16 / DWM_F16 / DWM_F32,
  * row pitch ld) -> out E4M3 [M, K] (pitch ldo bytes) and scale fp32 [M].  Per row:

@@ -344,11 +344,15 @@ bool attn_tcg_kv_eligible(const dwm_attention_args* a);
 int attn_wgmma_launch(const dwm_attention_args* a, cudaStream_t s);
 int attn_tcg_launch(const dwm_attention_args* a, cudaStream_t s);
 int attn_tcg_kv_launch(const dwm_attention_args* a, cudaStream_t s);
+bool attn_text_eligible(const dwm_attention_args* a);
+int attn_text_launch(const dwm_attention_args* a, bool causal, const float* bias, cudaStream_t s);
 
 }  // namespace dwm
 
-extern "C" int dwm_b200_attention(const dwm_attention_args* a, dwm_stream_t stream) {
-  using namespace dwm;
+namespace dwm {
+// text == true: dwm_b200_attention_text (causal / bias given, checked by the caller)
+static int attention_entry(const dwm_attention_args* a, bool text, bool causal, const float* bias,
+                           dwm_stream_t stream) {
   DWM_REQUIRE(a != nullptr, "dwm_b200_attention: null args");
   DWM_REQUIRE(a->head_dim == 64, "dwm_b200_attention: head_dim must be 64, got %d", a->head_dim);
   DWM_REQUIRE(a->qkv && a->out, "dwm_b200_attention: null qkv/out");
@@ -371,6 +375,17 @@ extern "C" int dwm_b200_attention(const dwm_attention_args* a, dwm_stream_t stre
     DWM_REQUIRE(a->ld_kv % 8 == 0 && a->k_col % 8 == 0 && a->v_col % 8 == 0 && a->seq_kv > 0 && a->inner_kv > 0 &&
                     (reinterpret_cast<uintptr_t>(a->kv) & 15) == 0,
                 "dwm_b200_attention: bad separate kv description");
+  if (text) {
+    // only the wgmma kernel has the causal mask and the additive bias
+    DWM_REQUIRE(causal != (bias != nullptr),
+                "dwm_b200_attention_text: give one of causal and bias (causal=%d, bias=%p)", int(causal),
+                static_cast<const void*>(bias));
+    DWM_REQUIRE(attn_text_eligible(a),
+                "dwm_b200_attention_text: needs contiguous sequences (group_strides[0] = inner = seq, unit "
+                "strides, one group dim) without mask, kv or split");
+    DWM_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 3) == 0, "dwm_b200_attention_text: bias must be 4-byte aligned");
+    return attn_text_launch(a, causal, bias, reinterpret_cast<cudaStream_t>(stream));
+  }
   {
     // contiguous sequences (joint / dual attention) and gathered unit sequences (cross-view /
     // temporal row-wise) run on the wgmma kernel; the rest (pointwise temporal, separate K,V,
@@ -412,4 +427,14 @@ extern "C" int dwm_b200_attention(const dwm_attention_args* a, dwm_stream_t stre
   if (a->dtype == DWM_F16) return launch_attn<__half>(p, s);
   set_last_error("dwm_b200_attention: dtype must be DWM_BF16 or DWM_F16, got %d", a->dtype);
   return -1;
+}
+}  // namespace dwm
+
+extern "C" int dwm_b200_attention(const dwm_attention_args* a, dwm_stream_t stream) {
+  return dwm::attention_entry(a, false, false, nullptr, stream);
+}
+
+extern "C" int dwm_b200_attention_text(const dwm_attention_args* a, int causal, const float* bias,
+                                       dwm_stream_t stream) {
+  return dwm::attention_entry(a, true, causal != 0, bias, stream);
 }

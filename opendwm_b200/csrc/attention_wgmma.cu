@@ -24,6 +24,11 @@
 // unsharded launch, and query unit u reads mask row mask_q0 + u, so each local query row sees
 // the same key blocks in the same order with the same arithmetic as its row of the unsharded
 // launch: its output is bit-identical.
+//
+// Text encoders (template flags CAUSAL, BIAS; contiguous sequences only): CLIP's causal mask
+// drops key j > query i; T5's relative-position bias [heads, seq, seq] (fp32, shared by every
+// group) is added to the scaled scores, which are then kept in log2 units, s*scale*log2(e) +
+// bias*log2(e), so the softmax below runs with a unit scale.
 #include <string.h>
 
 #include "common.cuh"
@@ -56,6 +61,7 @@ struct FaParams {
   // key / value columns of head 0 (in the qkv map, or in the K,V map with SKV), key units
   // (n_out without SKV) and the mask row of query unit 0
   int kcol, vcol, n_out_k, mask_q0;
+  const float* bias;   // BIAS: [heads, seq, seq]
 };
 
 // Descriptor of an MN-major operand (V: keys x head_dim, head_dim contiguous) written by TMA
@@ -76,12 +82,13 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-template <typename T, bool G, bool SKV>
+template <typename T, bool G, bool SKV, bool CAUSAL, bool BIAS>
 __global__ void __launch_bounds__(fa::THREADS, 1)
     attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_kv,
                       const FaParams p) {
   using namespace fa;
   static_assert(G || !SKV, "separate K,V needs gathered sequences");
+  static_assert(!G || (!CAUSAL && !BIAS), "causal / bias attention needs contiguous sequences");
   const CUtensorMap* kvmap = SKV ? &tmap_kv : &tmap;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sq = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // Q  [16 KB]
@@ -177,6 +184,7 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
     const int quad_col = 2 * (lane & 3);                       // first fragment column of this lane
     const int rows[2] = {cw * 64 + (warp & 3) * 16 + (lane >> 2), cw * 64 + (warp & 3) * 16 + (lane >> 2) + 8};
     const float sc = p.scale_log2;
+    const float sc_s = BIAS ? 1.0f : sc;   // scale still to apply to the (biased) scores
     const uint64_t dq = gmma_desc_sw128(smem_u32(sq + cw * 64 * 128));
     int kvs = 0, it = 0;
     uint32_t kvph = 0;
@@ -203,6 +211,18 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
             for (int ko = 0; ko < p.n_out_k; ++ko) al |= (__ldg(mr + ko) != 0 ? 1u : 0u) << ko;
             allowed[hi] = al;
           }
+        }
+      }
+      // CAUSAL / BIAS: sequence position of each row; a padding row (>= seq) reads the bias row
+      // of the last query, its output is never stored
+      int qpos[2] = {0, 0};
+      const float* brow[2] = {nullptr, nullptr};
+      if constexpr (CAUSAL || BIAS) {
+#pragma unroll
+        for (int hi = 0; hi < 2; ++hi) {
+          qpos[hi] = qt * BQ + rows[hi];
+          if constexpr (BIAS)
+            brow[hi] = p.bias + (static_cast<long long>(h) * p.seq + min(qpos[hi], p.seq - 1)) * p.seq;
         }
       }
       float o[32];
@@ -249,7 +269,7 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
           if (lane == 0) mbar_arrive(q_empty);
         }
         // ---- online softmax on the fragment: s[4j + e] = row rows[e >> 1], column 8j + quad_col + (e & 1)
-        const bool full = !G && kvalid >= BK;   // only the last block of a contiguous sequence is ragged
+        const bool full = !G && !CAUSAL && !BIAS && kvalid >= BK;   // only the last block of a contiguous sequence is ragged
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int j = 0; j < 16; ++j)
@@ -258,8 +278,11 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
             const int col = 8 * j + quad_col + (e & 1);
             const int hi = e >> 1;
             if (!full) {
-              const bool ok = G ? ((cmw[hi][col >> 5] >> (col & 31)) & 1u) != 0u : col < kvalid;
+              bool ok = G ? ((cmw[hi][col >> 5] >> (col & 31)) & 1u) != 0u : col < kvalid;
+              if constexpr (CAUSAL) ok = ok && kb * BK + col <= qpos[hi];
               if (!ok) s[4 * j + e] = -INFINITY;
+              else if constexpr (BIAS)
+                s[4 * j + e] = fmaf(s[4 * j + e], sc, __ldg(brow[hi] + kb * BK + col) * 1.4426950408889634f);
             }
             mx[hi] = fmaxf(mx[hi], s[4 * j + e]);
           }
@@ -268,7 +291,7 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
         for (int hi = 0; hi < 2; ++hi) {
           mx[hi] = fmaxf(mx[hi], __shfl_xor_sync(0xffffffffu, mx[hi], 1));
           mx[hi] = fmaxf(mx[hi], __shfl_xor_sync(0xffffffffu, mx[hi], 2));
-          const float m_new = fmaxf(m[hi], mx[hi] * sc);
+          const float m_new = fmaxf(m[hi], mx[hi] * sc_s);
           // a row whose keys were all masked so far (m_new = -inf, G only) keeps l = 0 / O = 0
           corr[hi] = m_new == -INFINITY ? 1.0f : ex2_approx(m[hi] - m_new);
           m[hi] = m_new;
@@ -285,7 +308,7 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
           float pv[4];
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            pv[e] = ex2_approx(fmaf(s[4 * j + e], sc, -mref[e >> 1]));
+            pv[e] = ex2_approx(fmaf(s[4 * j + e], sc_s, -mref[e >> 1]));
             l[e >> 1] += pv[e];
           }
           pa[j >> 1][(j & 1) * 2] = Cvt<T>::pack2(pv[0], pv[1]);
@@ -334,8 +357,8 @@ __global__ void __launch_bounds__(fa::THREADS, 1)
   }
 }
 
-template <typename T, bool G, bool SKV>
-static int launch_attn_wgmma(const dwm_attention_args* a, cudaStream_t s) {
+template <typename T, bool G, bool SKV, bool CAUSAL = false, bool BIAS = false>
+static int launch_attn_wgmma(const dwm_attention_args* a, cudaStream_t s, const float* bias = nullptr) {
   using namespace fa;
   FaParams p;
   memset(&p, 0, sizeof(p));
@@ -401,8 +424,9 @@ static int launch_attn_wgmma(const dwm_attention_args* a, cudaStream_t s) {
   p.out = a->out; p.ldo = a->ldo; p.out_group_stride = a->out_group_strides[0];
   p.split = a->split; p.out2 = a->out2; p.ldo2 = a->ldo2;
   p.scale_log2 = a->scale * 1.4426950408889634f;
+  p.bias = bias;
   if (!SKV) tm_kv = tm;
-  auto kern = attn_wgmma_kernel<T, G, SKV>;
+  auto kern = attn_wgmma_kernel<T, G, SKV, CAUSAL, BIAS>;
   static bool attr_set = false;
   if (!attr_set) {
     DWM_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
@@ -425,6 +449,17 @@ bool attn_tc_eligible(const dwm_attention_args* a) {
   return a->kv == nullptr && a->mask == nullptr && a->group_dims[1] == 1 && a->group_dims[2] == 1 &&
          a->inner == a->seq && a->stride_inner == 1 && a->out_stride_inner == 1 && a->seq > 64 &&
          a->group_strides[0] == a->seq && a->group_dims[0] * a->group_strides[0] < (1ll << 31);
+}
+
+// causal or biased attention (text encoders): the contiguous layout of attn_tc_eligible at any
+// seq >= 1 (a short sequence's 128-row tiles hold the next sequences' rows, which the key
+// mask drops and whose query rows are not stored), no split
+bool attn_text_eligible(const dwm_attention_args* a) {
+  return a->kv == nullptr && a->mask == nullptr &&
+         a->split == 0 && a->group_dims[1] == 1 && a->group_dims[2] == 1 && a->inner == a->seq &&
+         a->stride_inner == 1 && a->out_stride_inner == 1 && a->group_strides[0] == a->seq &&
+         a->group_dims[0] * a->group_strides[0] < (1ll << 31) &&
+         static_cast<long long>(a->heads) * a->seq * a->seq < (1ll << 31);
 }
 
 // gathered sequences of whole units of `inner` contiguous tokens (cross-view / temporal
@@ -475,6 +510,18 @@ int attn_wgmma_launch(const dwm_attention_args* a, cudaStream_t s) {
   if (a->dtype == DWM_F16) return launch_attn_wgmma<__half, false, false>(a, s);
   set_last_error("dwm_b200_attention: dtype must be DWM_BF16 or DWM_F16, got %d", a->dtype);
   return -1;
+}
+
+int attn_text_launch(const dwm_attention_args* a, bool causal, const float* bias, cudaStream_t s) {
+  const bool bf = a->dtype == DWM_BF16;
+  if (a->dtype != DWM_BF16 && a->dtype != DWM_F16) {
+    set_last_error("dwm_b200_attention: dtype must be DWM_BF16 or DWM_F16, got %d", a->dtype);
+    return -1;
+  }
+  if (causal) return bf ? launch_attn_wgmma<__nv_bfloat16, false, false, true, false>(a, s)
+                        : launch_attn_wgmma<__half, false, false, true, false>(a, s);
+  return bf ? launch_attn_wgmma<__nv_bfloat16, false, false, false, true>(a, s, bias)
+            : launch_attn_wgmma<__half, false, false, false, true>(a, s, bias);
 }
 
 int attn_tcg_launch(const dwm_attention_args* a, cudaStream_t s) {

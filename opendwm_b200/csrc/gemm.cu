@@ -181,7 +181,7 @@ int g_gemm_2cta = -1;   // -1: from env DWM_GEMM_2CTA (default 1), 0 / 1: forced
 // it saves a tenth of the waves x width, not for a smaller fraction of a wave that the tile
 // count rounds off: 4096 x 1536 x 1536 RESID picks 128 (1.1-1.3x), 2048 x 1536 keeps 256.
 static int pick_tile_n(const dwm_linear_args* a, int cl) {
-  if (a->epilogue == DWM_EPI_GEGLU) return 256;
+  if (a->epilogue == DWM_EPI_GEGLU || a->epilogue == DWM_EPI_GEGLU_TANH) return 256;
   if (g_gemm_bn == 128 || g_gemm_bn == 256) return g_gemm_bn;
   const long long slots = sm_count() / cl;
   const long long m_groups = ((a->M + BM - 1) / BM + cl - 1) / cl;
@@ -200,6 +200,11 @@ static int launch_pick_n(const dwm_linear_args* a, cudaStream_t s) {
 // 16-bit operands keep TF = T; E4M3 operands share one instantiation between both out_dtypes.
 template <typename TA, typename T, int CL, typename TF = T>
 static int dispatch_epi(const dwm_linear_args* a, cudaStream_t s) {
+  if constexpr (sizeof(TA) == 2) {   // text-encoder epilogues: 16-bit operands only
+    if (a->epilogue == DWM_EPI_STORE && a->act == DWM_ACT_QUICK_GELU)
+      return launch_pick_n<TA, T, EPI_STORE_QUICK_GELU, CL>(a, s);
+    if (a->epilogue == DWM_EPI_GEGLU_TANH) return launch_gemm<TA, T, DWM_EPI_GEGLU_TANH, 256, CL>(a, s);
+  }
   switch (a->epilogue) {
     case DWM_EPI_STORE: return launch_pick_n<TA, T, DWM_EPI_STORE, CL>(a, s);
     case DWM_EPI_GEGLU: return launch_gemm<TA, T, DWM_EPI_GEGLU, 256, CL>(a, s);
@@ -261,8 +266,14 @@ extern "C" int dwm_b200_linear(const dwm_linear_args* a, dwm_stream_t stream) {
               "dwm_b200_linear: A, W, out must be 16-byte aligned");
   DWM_REQUIRE(a->N % 32 == 0, "dwm_b200_linear: N must be a multiple of 32, got %lld", (long long)a->N);
   DWM_REQUIRE(a->ldo % 8 == 0, "dwm_b200_linear: ldo must be a multiple of 8");
-  if (a->epilogue == DWM_EPI_GEGLU)
+  if (a->epilogue == DWM_EPI_GEGLU || a->epilogue == DWM_EPI_GEGLU_TANH)
     DWM_REQUIRE(a->N % 256 == 0, "dwm_b200_linear: GEGLU needs N %% 256 == 0 (packed weight)");
+  if (a->epilogue == DWM_EPI_GEGLU_TANH || a->act == DWM_ACT_QUICK_GELU) {
+    DWM_REQUIRE(a->dtype == DWM_BF16 || a->dtype == DWM_F16,
+                "dwm_b200_linear: DWM_EPI_GEGLU_TANH and DWM_ACT_QUICK_GELU need 16-bit operands");
+    DWM_REQUIRE(a->act != DWM_ACT_QUICK_GELU || a->epilogue == DWM_EPI_STORE,
+                "dwm_b200_linear: DWM_ACT_QUICK_GELU needs the DWM_EPI_STORE epilogue");
+  }
   if (a->epilogue == DWM_EPI_QKNORM) {
     DWM_REQUIRE(a->N % 64 == 0 && a->qk_region > 0 && a->qk_region % 64 == 0 && a->q_norm_weight &&
                     (a->k_norm_weight || a->qk_norm_regions == 1),
@@ -270,7 +281,8 @@ extern "C" int dwm_b200_linear(const dwm_linear_args* a, dwm_stream_t stream) {
   }
   DWM_REQUIRE(a->n_peer_out >= 0 && a->n_peer_out <= 8, "dwm_b200_linear: n_peer_out out of range");
   if (a->n_peer_out > 0)
-    DWM_REQUIRE(a->epilogue == DWM_EPI_STORE || a->epilogue == DWM_EPI_QKNORM || a->epilogue == DWM_EPI_GEGLU,
+    DWM_REQUIRE(a->epilogue == DWM_EPI_STORE || a->epilogue == DWM_EPI_QKNORM || a->epilogue == DWM_EPI_GEGLU ||
+                    a->epilogue == DWM_EPI_GEGLU_TANH,
                 "dwm_b200_linear: peer_out needs a 16-bit epilogue");
   if (a->epilogue == DWM_EPI_RESID && a->blend_x)
     DWM_REQUIRE(a->alpha != nullptr, "dwm_b200_linear: blend_x without alpha");

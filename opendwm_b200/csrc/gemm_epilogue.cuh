@@ -17,6 +17,11 @@ constexpr int EPI_STAGE_BYTES = EPI_WARPS * 16 * 32 * 4;  // per consumer warp: 
 // register split (65536 per SM, one CTA): producer warpgroup 40, consumers 232 each
 constexpr int PRODUCER_REGS = 40;
 constexpr int CONSUMER_REGS = 232;
+// DWM_EPI_STORE with act = DWM_ACT_QUICK_GELU, compiled as an epilogue of its own so that the
+// run-time activation switch of DWM_EPI_STORE keeps its instructions
+constexpr int EPI_STORE_QUICK_GELU = 16;
+
+__device__ __forceinline__ float quick_gelu(float x) { return x / (1.0f + __expf(-1.702f * x)); }
 
 struct EpiParams {
   void* out;
@@ -118,7 +123,8 @@ template <typename T, int EPI, int NT>
 __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* stg, int m_base, int row0, int M,
                                            int n_tile0, int N, const EpiParams& p, int lane,
                                            const TileGeom geom = TileGeom{0, 0, 0, 0, 0}) {
-  constexpr bool kOut16 = (EPI == DWM_EPI_STORE || EPI == DWM_EPI_GEGLU || EPI == DWM_EPI_QKNORM);
+  constexpr bool kOut16 = (EPI == DWM_EPI_STORE || EPI == DWM_EPI_GEGLU || EPI == DWM_EPI_QKNORM ||
+                           EPI == EPI_STORE_QUICK_GELU || EPI == DWM_EPI_GEGLU_TANH);
   const int rs = lane >> 3;  // phase-2: row within a group of 4
   const int c4 = lane & 7;   // phase-2: float4 column within the 32-col chunk
 
@@ -222,7 +228,7 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
     }
   };
 
-  if constexpr (EPI == DWM_EPI_STORE || EPI == DWM_EPI_F32 || EPI == DWM_EPI_RESID) {
+  if constexpr (EPI == DWM_EPI_STORE || EPI == DWM_EPI_F32 || EPI == DWM_EPI_RESID || EPI == EPI_STORE_QUICK_GELU) {
     // fully unrolled: the fragment is indexed with compile-time offsets only
 #pragma unroll
     for (int c = 0; c < NT / 32; ++c) {
@@ -240,7 +246,10 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
           }
         }
         // activation selected once per chunk (warp-uniform), loops fully unrolled
-        if (p.act == DWM_ACT_GELU_TANH) {
+        if constexpr (EPI == EPI_STORE_QUICK_GELU) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) v[j] = quick_gelu(v[j]);
+        } else if (p.act == DWM_ACT_GELU_TANH) {
 #pragma unroll
           for (int j = 0; j < 16; ++j) v[j] = gelu_tanh(v[j]);
         } else if (p.act == DWM_ACT_SILU) {
@@ -255,9 +264,9 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
         }
       }
       stage_dump(stg, lane, v);
-      if constexpr (EPI == DWM_EPI_STORE) flush16(n0); else flush32(n0);
+      if constexpr (EPI == DWM_EPI_STORE || EPI == EPI_STORE_QUICK_GELU) flush16(n0); else flush32(n0);
     }
-  } else if constexpr (EPI == DWM_EPI_GEGLU) {
+  } else if constexpr (EPI == DWM_EPI_GEGLU || EPI == DWM_EPI_GEGLU_TANH) {
     static_assert(NT == 256, "GEGLU packs value / gate halves per 256-column tile");
     // tile columns [0,128) hold the value half, [128,256) the gate half of output
     // columns [n_tile0/2, n_tile0/2 + 128).
@@ -275,7 +284,7 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
           x += __ldg(bv + col);
           y += __ldg(bv + 128 + col);
         }
-        v[j] = x * gelu_erf(y);
+        v[j] = x * (EPI == DWM_EPI_GEGLU ? gelu_erf(y) : gelu_tanh(y));
       }
       stage_dump(stg, lane, v);
       flush16(n_tile0 / 2 + c * 32);

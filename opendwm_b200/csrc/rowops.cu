@@ -1,7 +1,7 @@
 // Memory-bound row / elementwise kernels of the CTSD step (sm_90a): LayerNorm with
 // AdaLN modulation (emits the 16-bit or row-scaled E4M3 GEMM operand), E4M3 row quantization,
 // activation casts, sinusoidal embeddings, patchify, and the fused CFG + un-patchify +
-// per-frame Euler update.
+// per-frame Euler update; the RMSNorm and the embedding gather of the text encoders.
 // All are single-pass over HBM with 128-bit accesses.
 #include "common.cuh"
 #include "../../include/dwm_b200.h"
@@ -517,6 +517,71 @@ __global__ void cfg_ddim_kernel(const float* __restrict__ pred, int cfg, float g
   (void)per_b;
 }
 
+// RMSNorm (T5LayerNorm) of one fp32 row per CTA: the sum of squares in fp32 (per-thread float4
+// partials, then a fixed-order warp / CTA reduction, so a row's result does not depend on the
+// batch), then out = weight * (x * rsqrt(mean + eps)) in the output type.
+constexpr int RMS_THREADS = 256;
+
+template <typename T>
+__device__ __forceinline__ void store4(T* dst, float a, float b, float c, float d) {
+  uint2 pk;
+  pk.x = Cvt<T>::pack2(a, b);
+  pk.y = Cvt<T>::pack2(c, d);
+  *reinterpret_cast<uint2*>(dst) = pk;
+}
+template <>
+__device__ __forceinline__ void store4<float>(float* dst, float a, float b, float c, float d) {
+  *reinterpret_cast<float4*>(dst) = make_float4(a, b, c, d);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(RMS_THREADS) rmsnorm_kernel(const float* __restrict__ x, long long ldx, int D,
+                                                              const float* __restrict__ w, float eps,
+                                                              T* __restrict__ out, long long ldo) {
+  __shared__ float red[RMS_THREADS / 32];
+  const float4* row = reinterpret_cast<const float4*>(x + static_cast<long long>(blockIdx.x) * ldx);
+  T* orow = out + static_cast<long long>(blockIdx.x) * ldo;
+  const int tid = threadIdx.x, nvec = D >> 2;
+  float ss = 0.f;
+  for (int i = tid; i < nvec; i += RMS_THREADS) {
+    const float4 v = row[i];
+    ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+  }
+  ss = warp_sum(ss);
+  if ((tid & 31) == 0) red[tid >> 5] = ss;
+  __syncthreads();
+  ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < RMS_THREADS / 32; ++i) ss += red[i];
+  const float r = rsqrtf(ss / static_cast<float>(D) + eps);
+  for (int i = tid; i < nvec; i += RMS_THREADS) {
+    const float4 v = row[i];
+    const float4 g = __ldg(reinterpret_cast<const float4*>(w) + i);
+    store4<T>(orow + 4 * i, g.x * (v.x * r), g.y * (v.y * r), g.z * (v.z * r), g.w * (v.w * r));
+  }
+}
+
+// out[m, :] = tok[ids[m], :] (+ pos[m % seq, :]): one fp32 add per element, as torch does it
+__global__ void embed_kernel(const long long* __restrict__ ids, long long M, long long seq,
+                             const float* __restrict__ tok, long long vocab, const float* __restrict__ pos,
+                             int D, float* __restrict__ out, long long ldo) {
+  const long long m = blockIdx.x;
+  const long long id = ids[m];
+  if (id < 0 || id >= vocab) __trap();   // token id outside the embedding table
+  const float4* t = reinterpret_cast<const float4*>(tok + id * D);
+  const float4* q = pos ? reinterpret_cast<const float4*>(pos + (m % seq) * D) : nullptr;
+  float4* o = reinterpret_cast<float4*>(out + m * ldo);
+  for (int i = threadIdx.x; i < (D >> 2); i += blockDim.x) {
+    float4 v = __ldg(t + i);
+    if (q) {
+      const float4 a = __ldg(q + i);
+      v.x = __fadd_rn(v.x, a.x); v.y = __fadd_rn(v.y, a.y); v.z = __fadd_rn(v.z, a.z); v.w = __fadd_rn(v.w, a.w);
+    }
+    o[i] = v;
+  }
+  (void)M;
+}
+
 // out[i] = s0[i / inner] * x[i] + s1[i / inner] * y[i]
 __global__ void lincomb2_kernel(const float* __restrict__ x, const float* __restrict__ y,
                                 const float* __restrict__ s0, const float* __restrict__ s1, long long n,
@@ -530,6 +595,45 @@ __global__ void lincomb2_kernel(const float* __restrict__ x, const float* __rest
 }  // namespace dwm
 
 using namespace dwm;
+
+extern "C" int dwm_b200_rmsnorm(const float* x, int64_t M, int64_t D, int64_t ldx, const float* weight, float eps,
+                                void* out, int64_t ldo, int dtype, dwm_stream_t stream) {
+  DWM_REQUIRE(x && weight && out, "dwm_b200_rmsnorm: null x/weight/out");
+  DWM_REQUIRE(M > 0 && M < (1ll << 31) && D > 0 && D % 4 == 0 && D < (1ll << 31) && ldx >= D && ldo >= D &&
+                  ldx % 4 == 0 && ldo % 4 == 0,
+              "dwm_b200_rmsnorm: need M > 0, D a multiple of 4, ldx / ldo >= D and multiples of 4; got M=%lld "
+              "D=%lld ldx=%lld ldo=%lld", (long long)M, (long long)D, (long long)ldx, (long long)ldo);
+  DWM_REQUIRE(is_aligned(x, 16) && is_aligned(weight, 16) && is_aligned(out, dtype == DWM_F32 ? 16 : 8),
+              "dwm_b200_rmsnorm: x, weight must be 16-byte and out 8-byte (fp32: 16-byte) aligned");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const unsigned grid = static_cast<unsigned>(M);
+  const int Di = static_cast<int>(D);
+  if (dtype == DWM_BF16)
+    rmsnorm_kernel<<<grid, RMS_THREADS, 0, s>>>(x, ldx, Di, weight, eps, static_cast<__nv_bfloat16*>(out), ldo);
+  else if (dtype == DWM_F16)
+    rmsnorm_kernel<<<grid, RMS_THREADS, 0, s>>>(x, ldx, Di, weight, eps, static_cast<__half*>(out), ldo);
+  else if (dtype == DWM_F32)
+    rmsnorm_kernel<<<grid, RMS_THREADS, 0, s>>>(x, ldx, Di, weight, eps, static_cast<float*>(out), ldo);
+  else
+    DWM_REQUIRE(false, "dwm_b200_rmsnorm: dtype must be DWM_BF16, DWM_F16 or DWM_F32, got %d", dtype);
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dwm_b200_embed(const int64_t* ids, int64_t M, int64_t seq, const float* tok, int64_t vocab,
+                              const float* pos, int64_t D, float* out, int64_t ldo, dwm_stream_t stream) {
+  DWM_REQUIRE(ids && tok && out, "dwm_b200_embed: null ids/tok/out");
+  DWM_REQUIRE(M > 0 && M < (1ll << 31) && seq > 0 && vocab > 0 && D > 0 && D % 4 == 0 && D < (1ll << 31) &&
+                  ldo >= D && ldo % 4 == 0,
+              "dwm_b200_embed: need M, seq, vocab > 0, D a multiple of 4, ldo >= D a multiple of 4");
+  DWM_REQUIRE(is_aligned(tok, 16) && is_aligned(pos, 16) && is_aligned(out, 16) && is_aligned(ids, 8),
+              "dwm_b200_embed: tok, pos, out must be 16-byte and ids 8-byte aligned");
+  const int threads = D >= 1024 ? 256 : 128;
+  embed_kernel<<<static_cast<unsigned>(M), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const long long*>(ids), M, seq, tok, vocab, pos, static_cast<int>(D), out, ldo);
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
 
 extern "C" int dwm_b200_lincomb2(const float* x, const float* y, const float* s0, const float* s1,
                                  int64_t n, int64_t inner, float* out, dwm_stream_t stream) {

@@ -10,8 +10,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdwm_b200.so")
 
 DWM_BF16, DWM_F16, DWM_F32, DWM_E4M3 = 0, 1, 2, 3
-ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU, ACT_RELU = 0, 1, 2, 3, 4
-EPI_STORE, EPI_GEGLU, EPI_QKNORM, EPI_RESID, EPI_F32 = 0, 1, 2, 3, 4
+ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU, ACT_RELU, ACT_QUICK_GELU = 0, 1, 2, 3, 4, 5
+EPI_STORE, EPI_GEGLU, EPI_QKNORM, EPI_RESID, EPI_F32, EPI_GEGLU_TANH = 0, 1, 2, 3, 4, 5
 
 _i64 = ctypes.c_int64
 _p = ctypes.c_void_p
@@ -102,7 +102,12 @@ SYMBOLS = {
     "dwm_b200_set_option": (ctypes.c_int, [ctypes.c_char_p, ctypes.c_int]),
     "dwm_b200_linear": (ctypes.c_int, [ctypes.POINTER(LinearArgs), _p]),
     "dwm_b200_attention": (ctypes.c_int, [ctypes.POINTER(AttentionArgs), _p]),
+    "dwm_b200_attention_text": (ctypes.c_int, [ctypes.POINTER(AttentionArgs), ctypes.c_int, _p,
+                                               _p]),
     "dwm_b200_layernorm": (ctypes.c_int, [ctypes.POINTER(LayerNormArgs), _p]),
+    "dwm_b200_rmsnorm": (ctypes.c_int, [_p, _i64, _i64, _i64, _p, ctypes.c_float, _p, _i64,
+                                        ctypes.c_int, _p]),
+    "dwm_b200_embed": (ctypes.c_int, [_p, _i64, _i64, _p, _i64, _p, _i64, _p, _i64, _p]),
     "dwm_b200_quantize_rows": (ctypes.c_int, [_p, _i64, _i64, _i64, ctypes.c_int, _p, _i64,
                                               _p, _p]),
     "dwm_b200_act_cast": (ctypes.c_int, [_p, _p, _i64, ctypes.c_int, ctypes.c_int, _p]),

@@ -153,7 +153,7 @@ def linear(a, w, bias=None, *, epilogue=_l.EPI_STORE, act=_l.ACT_NONE,
         if out_dtype not in (None, a.dtype):
             raise TypeError("16-bit operands write their own dtype, not {}".format(out_dtype))
         out16 = a.dtype
-    out_cols = N // 2 if epilogue == _l.EPI_GEGLU else N
+    out_cols = N // 2 if epilogue in (_l.EPI_GEGLU, _l.EPI_GEGLU_TANH) else N
     if out is None:
         if epilogue in (_l.EPI_RESID, _l.EPI_F32):
             out = torch.empty((M, out_cols), device=a.device, dtype=torch.float32)
@@ -251,7 +251,8 @@ def quantize_weight_rows(w):
 def pack_geglu(weight: torch.Tensor, bias=None, block=128):
     """Re-orders a diffusers GEGLU projection (rows [0,F) value, [F,2F) gate,
     FeedForward net.0.proj) into blocks [128 value | 128 gate] so one 256-column
-    GEMM tile holds matching value/gate columns."""
+    GEMM tile holds matching value/gate columns.  T5's gated GELU packs the same way
+    from cat([wi_1, wi_0]) (value wi_1, gate wi_0) for EPI_GEGLU_TANH."""
     two_f = weight.shape[0]
     f = two_f // 2
     if f % block:
@@ -278,9 +279,11 @@ def attention(qkv, out, *, D, heads, group_dims, group_strides, seq, inner=None,
               out_stride_outer=None, out_stride_inner=None, split=0, out2=None,
               mask=None, mask_div=1, scale=None, kv=None, k_col=0, v_col=0,
               kv_group_strides=None, seq_kv=None, inner_kv=None,
-              kv_stride_outer=0, kv_stride_inner=1, mask_q_offset=0):
+              kv_stride_outer=0, kv_stride_inner=1, mask_q_offset=0, causal=False, bias=None):
     """Gathered multi-head attention over the fused q|k|v buffer (or a separate
-    key/value buffer `kv`); see dwm_attention_args in include/dwm_b200.h."""
+    key/value buffer `kv`); see dwm_attention_args in include/dwm_b200.h.  Text encoders:
+    `causal` (CLIP) or `bias` fp32 [heads, seq, seq] added to the scaled scores (T5), on
+    contiguous sequences."""
     _rows2d(qkv, "qkv")
     _rows2d(out, "out")
     if not qkv.is_cuda:
@@ -323,6 +326,16 @@ def attention(qkv, out, *, D, heads, group_dims, group_strides, seq, inner=None,
         a.seq_kv = seq if seq_kv is None else seq_kv
         a.inner_kv = a.seq_kv if inner_kv is None else inner_kv
         a.kv_stride_outer, a.kv_stride_inner = kv_stride_outer, kv_stride_inner
+    if causal or bias is not None:
+        if bias is not None:
+            _f32(bias, "bias")
+            if tuple(bias.shape) != (heads, seq, seq) or not bias.is_contiguous():
+                raise ValueError("bias must be contiguous fp32 [heads, seq, seq] = [{}, {}, {}], "
+                                 "got {}".format(heads, seq, seq, list(bias.shape)))
+        _l.check(_l.load().dwm_b200_attention_text(ctypes.byref(a), int(bool(causal)),
+                                                   _ptr(bias), _stream()),
+                 "dwm_b200_attention_text")
+        return out
     _l.check(_l.load().dwm_b200_attention(ctypes.byref(a), _stream()),
              "dwm_b200_attention")
     return out
@@ -378,6 +391,42 @@ def layernorm(x, out, *, weight=None, bias=None, eps=1e-5, add_item=None,
         a.dtype = _dt(out)
     _l.check(_l.load().dwm_b200_layernorm(ctypes.byref(a), _stream()),
              "dwm_b200_layernorm")
+    return out
+
+
+def rmsnorm(x, weight, out, eps=1e-6):
+    """T5LayerNorm of an fp32 [M, D] stream: out = weight * x * rsqrt(mean(x^2) + eps), out
+    bf16 / fp16 (the GEMM operand) or fp32."""
+    _rows2d(_f32(x, "x"), "x")
+    _rows2d(out, "out")
+    _f32(weight, "weight")
+    M, D = x.shape
+    if weight.numel() != D or tuple(out.shape[:1]) != (M,) or out.shape[1] < D:
+        raise ValueError("rmsnorm: weight must be [D] and out [M, >= D]")
+    _l.check(_l.load().dwm_b200_rmsnorm(
+        x.data_ptr(), M, D, x.stride(0), weight.data_ptr(), float(eps), out.data_ptr(),
+        out.stride(0), _code(out.dtype), _stream()), "dwm_b200_rmsnorm")
+    return out
+
+
+def embed(ids, tok, out, pos=None, seq=None):
+    """out[m] = tok[ids[m]] (+ pos[m % seq]): the token / position embedding of a text
+    encoder into its fp32 residual stream out [M, D]; ids int64 [M] on the GPU."""
+    _f32(tok, "tok")
+    _f32(pos, "pos")
+    _rows2d(_f32(out, "out"), "out")
+    if ids.dtype != torch.int64 or ids.dim() != 1 or not ids.is_contiguous() or not ids.is_cuda:
+        raise TypeError("ids must be a contiguous cuda int64 [M] tensor")
+    M, D = out.shape
+    if ids.numel() != M or tok.dim() != 2 or tok.shape[1] != D or not tok.is_contiguous():
+        raise ValueError("embed: ids [M], tok [vocab, D] and out [M, D] must agree")
+    seq = M if seq is None else seq
+    if pos is not None and (tuple(pos.shape[1:]) != (D,) or pos.shape[0] < seq or
+                            not pos.is_contiguous()):
+        raise ValueError("embed: pos must be contiguous [>= seq, D]")
+    _l.check(_l.load().dwm_b200_embed(
+        ids.data_ptr(), M, seq, tok.data_ptr(), tok.shape[0], _ptr(pos), D, out.data_ptr(),
+        out.stride(0), _stream()), "dwm_b200_embed")
     return out
 
 

@@ -289,7 +289,8 @@ class CrossviewTemporalSD:
             from dwm.pipelines.text_conditions import load_text_encoders
             loaded = load_text_encoders(
                 self.is_dit, self._text_pending, self.device,
-                common_config.get("text_encoder_load_args", {}))
+                common_config.get("text_encoder_load_args", {}),
+                native=common_config.get("native_text_encoders", False))
             if loaded is not None:
                 self.text_encoders, self.tokenizers = loaded
         if not self.is_dit and not isinstance(

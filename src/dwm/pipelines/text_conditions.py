@@ -1,12 +1,13 @@
 """Prompt -> text-condition tensors for `CrossviewTemporalSD.get_conditions`.
 
-The text encoders are callers of the hot path (SURVEY.md §8 A13): they run once per window
-through Hugging Face `transformers`, exactly as in the reference
+The text encoders are callers of the hot path (SURVEY.md §8 A13): by default they run through
+Hugging Face `transformers`, exactly as in the reference
 (src/dwm/pipelines/ctsd.py:39-83 `flatten_clip_text`, :176-253 the text branch of
 `get_conditions`, :744-805 the SD-3 prompt encoders, :886-948 loading).  This module is the
 thin adapter that lets reference-style batches (`clip_text` = nested prompt lists) drive the
 H100 pipeline when the encoder weights are present; batches that carry pre-encoded
-`text_embeddings` / `pooled_text_embeddings` bypass it.
+`text_embeddings` / `pooled_text_embeddings` bypass it.  With `native=True` the same calls run
+on dwm.models.text_encoders (the sm_90a kernels).
 """
 import os
 
@@ -97,28 +98,40 @@ def text_conditions(is_dit: bool, text_encoder, tokenizer, clip_text, sequence_l
     return spread(states), (spread(pooled) if is_dit else None)
 
 
-def load_text_encoders(is_dit: bool, path: str, device, load_args: dict):
+def load_text_encoders(is_dit: bool, path: str, device, load_args: dict, native: bool = False):
     """(text_encoder(s), tokenizer(s)) from a diffusers-layout checkpoint directory, or None
-    when it does not hold them (then conditions must come pre-encoded)."""
+    when it does not hold them (then conditions must come pre-encoded).  native=True loads the
+    encoders as dwm.models.text_encoders (the sm_90a kernels, from safetensors weights, with
+    load_args' torch_dtype as the dtype of the states they return); tokenizers stay
+    transformers on the CPU."""
     import transformers
 
     def has(sub):
         return path is not None and os.path.isdir(os.path.join(path, sub))
     if not has("tokenizer") or not has("text_encoder"):
         return None
-    frozen = lambda m: m.requires_grad_(False).eval()   # noqa: E731
+    if native:
+        from dwm.models import text_encoders as te
+        dtype = load_args.get("torch_dtype", load_args.get("dtype"))
+
+        def load(cls, sub):
+            return cls.from_pretrained(path, subfolder=sub, device=device, torch_dtype=dtype)
+        clip, clip_proj, t5 = (te.NativeCLIPTextModel, te.NativeCLIPTextModelWithProjection,
+                               te.NativeT5EncoderModel)
+    else:
+        frozen = lambda m: m.requires_grad_(False).eval()   # noqa: E731
+
+        def load(cls, sub):
+            return frozen(cls.from_pretrained(path, subfolder=sub, **load_args)).to(device)
+        clip, clip_proj, t5 = (transformers.CLIPTextModel,
+                               transformers.CLIPTextModelWithProjection,
+                               transformers.T5EncoderModel)
     if not is_dit:
         tok = transformers.CLIPTokenizer.from_pretrained(path, subfolder="tokenizer")
-        enc = transformers.CLIPTextModel.from_pretrained(path, subfolder="text_encoder",
-                                                         **load_args)
-        return frozen(enc).to(device), tok
+        return load(clip, "text_encoder"), tok
     toks = [transformers.CLIPTokenizer.from_pretrained(path, subfolder="tokenizer"),
             transformers.CLIPTokenizer.from_pretrained(path, subfolder="tokenizer_2"),
             transformers.T5TokenizerFast.from_pretrained(path, subfolder="tokenizer_3")]
-    encs = [frozen(transformers.CLIPTextModelWithProjection.from_pretrained(
-        path, subfolder=sub, **load_args)).to(device)
-        for sub in ("text_encoder", "text_encoder_2")]
-    encs.append(frozen(transformers.T5EncoderModel.from_pretrained(
-        path, subfolder="text_encoder_3", **load_args)).to(device)
-        if has("text_encoder_3") else None)
+    encs = [load(clip_proj, sub) for sub in ("text_encoder", "text_encoder_2")]
+    encs.append(load(t5, "text_encoder_3") if has("text_encoder_3") else None)
     return encs, toks
