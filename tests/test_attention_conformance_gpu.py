@@ -17,12 +17,20 @@ layout.  Every GPU case therefore:
     it says wgmma (so a case meant for the wgmma kernel cannot quietly test mma.sync twice);
   * repeats the attn_tc = 2 call, which must give identical bits.
 
-The CPU self-test checks the bound itself against an emulated kernel and three wrong ones.
+Causal (CLIP) and biased (T5) attention, `dwm_b200_attention_text`, runs one kernel,
+attn_wgmma_kernel<T, false, false, CAUSAL, BIAS>, under every attn_tc setting: its cases run
+under attn_tc = 0 and 2 and must give the same bits, and `check_text_attention_selection` checks
+with torch.profiler that the kernel launched carries the expected flags.
+
+The CPU self-test checks the bound itself against an emulated kernel and seven wrong ones.
 """
+import re
 import math
 
 import pytest
 import torch
+
+from test_gemm_conformance_gpu import run_isolated
 
 SENTINEL = -21555     # int16 0xABCD: the bits of every output element the call must not write
 GUARD = 3             # sentinel rows before and after each output buffer
@@ -47,9 +55,11 @@ class Layout:
 
     def __init__(self, heads, group_dims, group_strides, seq, inner=None, stride_outer=0,
                  stride_inner=1, out_group_strides=None, out_stride_outer=None,
-                 out_stride_inner=None, split=0, mask=None, mask_div=1, tail=5):
+                 out_stride_inner=None, split=0, mask=None, mask_div=1, tail=5, scale=0.125,
+                 causal=False, bias=None):
         pad = lambda v, fill: list(v) + [fill] * (3 - len(v))  # noqa: E731
         self.heads, self.seq, self.split = heads, seq, split
+        self.scale, self.causal, self.bias = scale, causal, bias
         self.gd, self.gs = pad(group_dims, 1), pad(group_strides, 0)
         self.inner = seq if inner is None else inner
         self.so, self.si = stride_outer, stride_inner
@@ -90,12 +100,23 @@ class Layout:
                   out_stride_inner=self.osi, split=self.split, mask_div=self.mask_div)
         if self.mask is not None:
             kw["mask"] = self.mask.to(torch.uint8).cuda().contiguous()
+        if self.text:
+            kw.update(scale=self.scale, causal=self.causal,
+                      bias=None if self.bias is None else self.bias.float().cuda().contiguous())
         return kw
+
+    @property
+    def text(self):
+        return self.causal or self.bias is not None
 
     def kernel_path(self):
         """Which kernel attn_tc >= 1 selects: "tc" (wgmma, 2-D tensor map), "tcg" (wgmma, 5-D
         gathered tensor map) or "mma" (attention.cu).  Restates attn_tc_eligible and
-        attn_tcg_eligible of attention_wgmma.cu for calls without a separate kv."""
+        attn_tcg_eligible of attention_wgmma.cu for calls without a separate kv.  Causal or
+        biased calls ("text") run attn_wgmma_kernel<T, false, false, CAUSAL, BIAS> whatever
+        attn_tc says."""
+        if self.text:
+            return "text"
         gd, gs, ogs = self.gd, self.gs, self.ogs
         if (self.mask is None and gd[1] == 1 and gd[2] == 1 and self.inner == self.seq and
                 self.si == 1 and self.osi == 1 and self.seq > 64 and gs[0] == self.seq and
@@ -117,10 +138,11 @@ class Layout:
         return "tcg"
 
 
-def contiguous(heads, N, seq, pad=0, out_pad=None, split=0):
-    """N contiguous sequences `pad` rows apart (joint / dual / UNet spatial attention)."""
+def contiguous(heads, N, seq, pad=0, out_pad=None, split=0, **text):
+    """N contiguous sequences `pad` rows apart (joint / dual / UNet spatial attention; with
+    `text` = scale / causal / bias, the text encoders' attention)."""
     ogs = None if out_pad is None else [seq + out_pad]
-    return Layout(heads, [N], [seq + pad], seq, out_group_strides=ogs, split=split)
+    return Layout(heads, [N], [seq + pad], seq, out_group_strides=ogs, split=split, **text)
 
 
 def crossview(heads, BT, H, V, W, *, unit_pad=0, group_pad=0, out="same", mask=None,
@@ -178,25 +200,37 @@ def gather_qkv(qkv, rows, heads):
     return x.permute(2, 0, 3, 1, 4)
 
 
-def reference(q, k, v, scale, mask=None):
-    """float64 (softmax(q k^T scale) v, softmax(q k^T scale) |v|) for q, k, v [G, H, S, 64]
-    and mask bool [G, S, S] (True = attend).  A query whose every key is masked gives 0 in
-    both (the kernels' contract, include/dwm_b200.h)."""
+def causal_mask(S, shift=0):
+    """bool [S, S]: query i attends keys j <= i + shift (CLIP's causal mask at shift 0)."""
+    return torch.ones(S, S, dtype=torch.bool).tril(shift)
+
+
+def reference(q, k, v, scale, mask=None, causal=False, bias=None):
+    """float64 (softmax(q k^T scale + bias) v, the same softmax applied to |v|, the sum of |v|
+    over each query's attended keys) for q, k, v [G, H, S, 64], mask bool [G, S, S] (True =
+    attend), `causal` (key j > query i dropped) and bias [H, S, S] (added after the scale, as
+    the kernel does).  A query whose every key is masked gives 0 in all three (the kernels'
+    contract, include/dwm_b200.h)."""
     q, k, v = q.double(), k.double(), v.double()
     s = q @ k.transpose(-1, -2) * scale
+    if bias is not None:
+        s = s + bias.double().to(s.device)[None]
     if mask is not None:
         s = s.masked_fill(~mask[:, None].to(s.device), float("-inf"))
+    if causal:
+        s = s.masked_fill(~causal_mask(s.shape[-1]).to(s.device), float("-inf"))
     m = s.amax(-1, keepdim=True)
     e = torch.exp(s - torch.where(torch.isfinite(m), m, torch.zeros_like(m)))
     l = e.sum(-1, keepdim=True)
     p = e / torch.where(l > 0, l, torch.ones_like(l))
-    return p @ v, p @ v.abs()
+    return p @ v, p @ v.abs(), torch.isfinite(s).double() @ v.abs()
 
 
-def bound_violations(out, ref, pv_abs, u):
-    """Elements of `out` outside |out - ref| <= u |ref| + 2u (P|V|) + 1e-6 (P|V|), and the worst
-    ratio |out - ref| / bound.  P|V| is the float64 softmax applied to |V|: the weighted mean
-    of the attended |v| for that query, head and column.
+def bound_violations(out, ref, pv_abs, u, v_sum=None):
+    """Elements of `out` outside |out - ref| <= u |ref| + 2u (P|V|) + 1e-6 (P|V|) (+ 2^-24 sum|v|
+    in fp16), and the worst ratio |out - ref| / bound.  P|V| is the float64 softmax applied to
+    |V|: the weighted mean of the attended |v| for that query, head and column; sum|v| (`v_sum`)
+    the plain sum of the attended |v|.
 
     The bound follows from where a kernel rounds (u = unit roundoff: 2^-8 bf16, 2^-11 fp16):
       * P is rounded to 16 bits for the P.V MMA: each p_j moves by at most u p_j, so the
@@ -207,16 +241,24 @@ def bound_violations(out, ref, pv_abs, u):
         accumulation, whose relative errors (~2^-22) are far smaller;
       * the output is rounded to 16 bits once: at most u |ref| (plus u times the errors above);
       * 1e-6 (P|V|) covers fp16 P values below 2^-14 that round to subnormals, whose absolute
-        error 2^-25 is not relative to p.
+        error 2^-25 is not relative to p.  That holds while the keys with such p carry |v| like
+        the winners'.  With `v_sum`, fp16 also gets 2^-24 sum|v|: every unnormalised p_j <=
+        2^(1/16) (see below) moves by at most 2^-25 absolutely and l >= 2^(-1/16), so this
+        bounds them whatever their |v|.  The unscaled T5 logits (std ~10 and more) put most
+        keys there.
     A query whose every key is masked has ref = P|V| = 0, so it must come out exactly 0.
 
     Worst ratio over this file's cases, measured on an H100 80GB HBM3 (bf16 / fp16):
     mma.sync 0.43 / 0.46; wgmma 0.63 / 0.65, both in the case where one key wins by 2^20.
+    The text kernel (causal / biased, on an H100 80GB HBM3 at a 700 W power limit): 0.60 / 0.62
+    on the random-data cases, 0.63 / 0.64 on the logit extremes.
     There the wgmma kernel's running max is the fp32 product max*scale while p is
     ex2(fma(s, scale, -max)), so the winner's p is 2^(+-1/16), not 1: its 16-bit rounding then
     costs the full u (P|V|) above, on top of the output's u |ref|."""
     out = out.double()
     tol = u * ref.abs() + (2 * u + 1e-6) * pv_abs
+    if v_sum is not None and u == 2.0 ** -11:
+        tol = tol + 2.0 ** -24 * v_sum
     err = (out - ref).abs()
     bad = ~(err <= tol)                         # NaN / Inf in out count as violations
     ratio = torch.where(err == 0, 0.0, err / tol)
@@ -224,11 +266,16 @@ def bound_violations(out, ref, pv_abs, u):
     return bad, ratio.max().item() if ratio.numel() else 0.0
 
 
-def emulate(q, k, v, scale, dtype, mask=None, block=128, drop_last_block=False):
+def emulate(q, k, v, scale, dtype, mask=None, block=128, drop_last_block=False, causal=False,
+            bias=None):
     """fp32 online softmax over key blocks as both kernels compute it: running max, P rounded
-    to `dtype` before P.V, l summed from the unrounded p, the output rounded to `dtype` once."""
+    to `dtype` before P.V, l summed from the unrounded p, the output rounded to `dtype` once;
+    `causal` / `bias` [H, S, S] as `reference` takes them."""
     q, k, v = q.float(), k.float(), v.float()
     G, H, S, _ = q.shape
+    if causal:
+        cm = causal_mask(S).expand(G, S, S)
+        mask = cm if mask is None else mask & cm
     m = torch.full((G, H, S, 1), float("-inf"))
     l = torch.zeros(G, H, S, 1)
     o = torch.zeros(G, H, S, 64)
@@ -236,6 +283,8 @@ def emulate(q, k, v, scale, dtype, mask=None, block=128, drop_last_block=False):
     for b in range(n_blocks):
         sl = slice(b * block, (b + 1) * block)
         s = q @ k[:, :, sl].transpose(-1, -2) * scale
+        if bias is not None:
+            s = s + bias.float()[None, :, :, sl]
         if mask is not None:
             s = s.masked_fill(~mask[:, None, :, sl], float("-inf"))
         m_new = torch.maximum(m, s.amax(-1, keepdim=True))
@@ -256,7 +305,12 @@ def test_bound_accepts_emulated_kernel_and_rejects_wrong_ones(dtype):
     """The bound passes an emulated kernel and fails each of three plausible kernel bugs:
     a dropped last key block, the scale 1/sqrt(65) for 1/sqrt(64), and keys / values read one
     row off in a gathered layout.  Cross-view layout, seq 4 x 48 = 192 (two key blocks), a
-    mask with fully masked rows, queries of std 2 (logits of std ~2)."""
+    mask with fully masked rows, queries of std 2 (logits of std ~2).
+
+    Then the text path, 3 contiguous sequences of 150 tokens (two key blocks), 2 heads: the
+    emulated causal and biased kernels pass, and four wrong ones fail: the causal mask
+    shifted by one key, the bias transposed ([h, j, i]), the bias of head h + 1, and the bias
+    multiplied by the scale (0.125 here: at T5's scale 1 that bug is invisible)."""
     lay = crossview(2, BT=2, H=2, V=4, W=48, unit_pad=3,
                     mask=unit_mask("empty", 2, 4, seed=1), mask_div=1)
     g = torch.Generator().manual_seed(0)
@@ -266,7 +320,7 @@ def test_bound_accepts_emulated_kernel_and_rejects_wrong_ones(dtype):
     u = unit_roundoff(dtype)
     mask = lay.mask_bool()
     q, k, v = gather_qkv(qkv, lay.in_rows, 2)
-    ref, pv = reference(q, k, v, 0.125, mask)
+    ref, pv, _ = reference(q, k, v, 0.125, mask)
     assert (~mask).all(-1).any(), "the case must have fully masked queries"
 
     bad, worst = bound_violations(emulate(q, k, v, 0.125, dtype, mask), ref, pv, u)
@@ -282,6 +336,27 @@ def test_bound_accepts_emulated_kernel_and_rejects_wrong_ones(dtype):
     for name, out in wrong.items():
         bad, worst = bound_violations(out, ref, pv, u)
         assert bad.any(), (name, worst)
+
+    lay = contiguous(2, 3, 150)
+    q, k, v = gather_qkv(torch.randn(lay.n_rows, 3 * 128, generator=g).to(dtype), lay.in_rows, 2)
+    bias = torch.randn(2, 150, 150, generator=g) * 3
+    S = lay.seq
+    for causal, b, wrong in [
+            (True, None, {"causal mask shifted by one key":
+                          dict(mask=causal_mask(S, 1).expand(lay.G, S, S))}),
+            (False, bias, {"bias transposed": dict(bias=bias.transpose(1, 2)),
+                           "bias of head h + 1": dict(bias=bias.roll(-1, 0)),
+                           "bias multiplied by the scale": dict(bias=bias * 0.125)})]:
+        ref, pv, vs = reference(q, k, v, 0.125, causal=causal, bias=b)
+        bad, worst = bound_violations(emulate(q, k, v, 0.125, dtype, causal=causal, bias=b), ref, pv, u, vs)
+        assert not bad.any(), ("causal" if causal else "bias", worst)
+        assert worst > 0.05, worst
+        for name, kw in wrong.items():
+            kw = dict(dict(causal=causal, bias=b), **kw)
+            if "mask" in kw:
+                kw["causal"] = False
+            bad, worst = bound_violations(emulate(q, k, v, 0.125, dtype, **kw), ref, pv, u, vs)
+            assert bad.any(), (name, worst)
 
 
 # --------------------------------------------------------------------------------------------
@@ -384,7 +459,8 @@ def _make_qkv(lay, dtype, seed):
 
 
 def _launch(lay, qkv, dtype, tc):
-    """One call into sentinel-filled buffers; returns (buf, buf2) including the guard bands."""
+    """One call into sentinel-filled buffers; returns (buf, buf2) including the guard bands.
+    Text layouts pass scale / causal / bias through lay.kwargs()."""
     from opendwm_b200 import lib, ops
     D = lay.heads * 64
 
@@ -409,7 +485,7 @@ def _written(buf, rows, D):
     return w
 
 
-def _check(lay, bufs, ref, pv, u, what):
+def _check(lay, bufs, ref, pv, u, what, vs=None):
     """Sentinel bits outside the write set; finite values within the bound inside it."""
     D = lay.heads * 64
     buf, buf2 = bufs
@@ -423,7 +499,7 @@ def _check(lay, bufs, ref, pv, u, what):
         stray = b.view(torch.int16)[~w] != SENTINEL
         assert not stray.any(), "%s: %d element(s) written outside the output" % (what, stray.sum())
         got[:, js] = b[(rows + GUARD).to(b.device)][..., :D]
-    bad, worst = bound_violations(got, ref, pv, u)
+    bad, worst = bound_violations(got, ref, pv, u, vs)
     if bad.any():
         g, j, d = (int(i) for i in bad.nonzero()[0])
         raise AssertionError(
@@ -435,34 +511,38 @@ def _check(lay, bufs, ref, pv, u, what):
 
 
 def _reference(lay, qkv):
-    """float64 (ref, P|V|) as [G, seq, D], computed a few groups at a time."""
+    """float64 (ref, P|V|, sum|v|) as [G, seq, D], computed a few groups at a time."""
     mask = lay.mask_bool()
     step = max(1, (1 << 25) // (lay.heads * lay.seq * lay.seq))
-    refs, pvs = [], []
+    outs = []
     for g0 in range(0, lay.G, step):
         q, k, v = gather_qkv(qkv, lay.in_rows[g0:g0 + step], lay.heads)
-        r, p = reference(q, k, v, 0.125, None if mask is None else mask[g0:g0 + step])
-        refs.append(r)
-        pvs.append(p)
+        outs.append(reference(q, k, v, lay.scale, None if mask is None else mask[g0:g0 + step],
+                              lay.causal, lay.bias))
     flat = lambda t: torch.cat(t).transpose(1, 2).reshape(lay.G, lay.seq, -1)  # noqa: E731
-    return flat(refs), flat(pvs)
+    return tuple(flat([o[i] for o in outs]) for i in range(3))
 
 
 def _conform(lay, qkv, dtype, distinct=True):
     """Both kernels against float64, the dispatch check and the repeat; returns the worst
     bound ratio of each run."""
     u = unit_roundoff(dtype)
-    ref, pv = _reference(lay, qkv)
+    ref, pv, vs = _reference(lay, qkv)
+    # the text kernel's fp16 P underflows for most keys (see bound_violations); elsewhere the
+    # bound stays as it was measured
+    vs = vs if lay.text else None
     path = lay.kernel_path()
     b0 = _launch(lay, qkv, dtype, 0)
     b2 = _launch(lay, qkv, dtype, 2)
     b2r = _launch(lay, qkv, dtype, 2)
-    r0 = _check(lay, b0, ref, pv, u, "attn_tc=0 (mma.sync)")
-    r2 = _check(lay, b2, ref, pv, u, "attn_tc=2 (%s)" % path)
+    r0 = _check(lay, b0, ref, pv, u, "attn_tc=0 (%s)" % ("text" if lay.text else "mma.sync"), vs)
+    r2 = _check(lay, b2, ref, pv, u, "attn_tc=2 (%s)" % path, vs)
     bits = lambda b: [x.view(torch.int16) for x in b if x is not None]  # noqa: E731
     assert all(torch.equal(x, y) for x, y in zip(bits(b2), bits(b2r))), "not repeatable"
     same = all(torch.equal(x, y) for x, y in zip(bits(b0), bits(b2)))
-    if path == "mma":
+    if path == "text":
+        assert same, "causal / biased attention gave other bits under attn_tc=0 and attn_tc=2"
+    elif path == "mma":
         assert same, "the layout is not wgmma-eligible, yet attn_tc=2 ran another kernel"
     elif distinct and lay.G * lay.seq * lay.heads * 64 >= 64 * 64:
         assert not same, ("the layout is %s-eligible, yet attn_tc=2 gave the mma.sync kernel's "
@@ -526,3 +606,156 @@ def test_attention_logit_extremes(layout, kind, dtype):
     assert lay.kernel_path() == ("tc" if layout == "contig" else "tcg")
     qkv = _extreme(_make_qkv(lay, dtype, seed=9), lay, kind)
     _conform(lay, qkv, dtype, distinct=False)
+
+
+# --------------------------------------------------------------------------------------------
+# text encoders: causal (CLIP) and biased (T5) attention on contiguous sequences
+# --------------------------------------------------------------------------------------------
+TEXT_SEQS = [1, 63, 64, 65, 77, 127, 128, 129, 300]
+TEXT_HEADS = [12, 20, 64]
+
+
+def _text_bias(heads, seq, seed, std=3.0):
+    return torch.randn(heads, seq, seq, generator=torch.Generator().manual_seed(seed)) * std
+
+
+def _text_layout(mode, seq, heads, G, seed, out_pad=None):
+    """`mode` "causal" (CLIP, scale 1/8) or "bias" (T5: unscaled, but scale 1/8 at 20 heads so
+    that a kernel scaling the bias too is caught)."""
+    if mode == "causal":
+        return contiguous(heads, G, seq, out_pad=out_pad, causal=True)
+    return contiguous(heads, G, seq, out_pad=out_pad, scale=0.125 if heads == 20 else 1.0,
+                      bias=_text_bias(heads, seq, seed))
+
+
+def _text_cases():
+    cases = []
+    for mode in ("causal", "bias"):
+        for seq in TEXT_SEQS:
+            for heads in TEXT_HEADS:
+                cases.append(("%s_s%d_h%d_g3" % (mode, seq, heads), mode, seq, heads, 3))
+        # a CFG window's prompt batch: 192 prompts of 77 tokens, several waves of 128-row
+        # tiles that straddle the sequences
+        for heads in (12, 20):
+            cases.append(("%s_s77_h%d_g192" % (mode, heads), mode, 77, heads, 192))
+    return cases
+
+
+TEXT_CASES = _text_cases()
+
+
+@pytest.mark.gpu
+@DTYPES
+@pytest.mark.parametrize("name,mode,seq,heads,G", TEXT_CASES, ids=[c[0] for c in TEXT_CASES])
+def test_text_attention_conforms(name, mode, seq, heads, G, dtype):
+    """q|k|v with ld = 3D + 8 poisoned columns and poisoned rows after the last sequence; the
+    cases with an odd seq + heads write their sequences 3 rows apart (sentinel rows between)."""
+    lay = _text_layout(mode, seq, heads, G, seed=seq * 131 + heads,
+                       out_pad=3 if (seq + heads) % 2 else None)
+    assert lay.kernel_path() == "text"
+    r0, r2 = _conform(lay, _make_qkv(lay, dtype, seed=seq + heads), dtype)
+    print("BOUND_RATIO attention_text %s_%s %.4g" % (name, dtype, max(r0, r2)))
+
+
+def _text_extreme(lay, qkv, kind):
+    """The EXTREMES on the text path.  Causal: as `_extreme` makes them.  Bias (unscaled, as in
+    T5): the bias carries the extreme where it can: "dominant" adds 2^20 to one key of every
+    row, "pm80" makes every logit bias +-80 (the losers' exp underflows fp32), "uniform" and
+    "zero_q" keep a bias that is constant along each row (uniform P) or only the bias (zero q).
+    "pad_mask" adds -1e9, as a padding mask does, to every fifth key and the last 7 keys of each
+    row: their P must be exactly 0.  A row whose every key is so masked would be a uniform
+    softmax in float64 and is out of scope."""
+    H, S = lay.heads, lay.seq
+    g = torch.Generator().manual_seed(17)
+    if lay.causal:
+        return lay, _extreme(qkv, lay, kind)
+    b = _text_bias(H, S, seed=S)
+    if kind in ("uniform", "zero_q"):
+        qkv = _extreme(qkv, lay, kind)
+        b = b[:, :, :1].expand(H, S, S).contiguous() if kind == "uniform" else b
+    elif kind == "dominant":
+        b[:, :, (2 * S) // 3] = 2.0 ** 20
+    elif kind == "pm80":
+        b = 80.0 * (torch.randint(0, 2, (H, S, S), generator=g) * 2 - 1) + 0.5 * torch.randn(H, S, S, generator=g)
+    else:
+        j = torch.arange(S)
+        b[:, :, (j % 5 == 0) | (j >= S - 7)] = -1e9
+    lay.bias = b
+    return lay, qkv
+
+
+TEXT_EXTREMES = [("causal", k) for k in EXTREMES] + [("bias", k) for k in EXTREMES + ["pad_mask"]]
+
+
+@pytest.mark.gpu
+@DTYPES
+@pytest.mark.parametrize("mode,kind", TEXT_EXTREMES, ids=["%s_%s" % c for c in TEXT_EXTREMES])
+def test_text_attention_logit_extremes(mode, kind, dtype):
+    """3 sequences of 129 tokens (a 1-row second tile), 4 heads, T5's scale 1 for the bias; the
+    padding mask is a bias, so it has no causal case."""
+    lay = contiguous(4, 3, 129, causal=mode == "causal", scale=0.125 if mode == "causal" else 1.0,
+                     bias=None if mode == "causal" else torch.zeros(4, 129, 129))
+    lay, qkv = _text_extreme(lay, _make_qkv(lay, dtype, seed=21), kind)
+    r0, r2 = _conform(lay, qkv, dtype, distinct=False)
+    print("BOUND_RATIO attention_text_extremes %s_%s_%s %.4g" % (mode, kind, dtype, max(r0, r2)))
+
+
+def _attn_launched(fn):
+    """(T, G, SKV, CAUSAL, BIAS) of every attn_wgmma_kernel `fn` launches, in order."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    found = []
+    for ev in prof.events():
+        m = re.search(r"attn_wgmma_kernel<(.*)>", ev.name)
+        if m:
+            args = [re.sub(r"^\((int|bool)\)", "", a.strip()) for a in m.group(1).split(",")]
+            found.append((args[0].split("::")[-1],) + tuple(a in ("true", "1") for a in args[1:5]))
+    return found
+
+
+@pytest.mark.gpu
+def test_text_attention_selection():
+    """check_text_attention_selection, in a process of its own (run_isolated)."""
+    run_isolated("test_attention_conformance_gpu", "check_text_attention_selection")
+
+
+def check_text_attention_selection():
+    """Causal and biased calls launch attn_wgmma_kernel<T, false, false, CAUSAL, BIAS> with the
+    flags of the call, in both dtypes, under every attn_tc setting, at a short sequence (which
+    the plain path would send to mma.sync) and a long one."""
+    from opendwm_b200 import lib, ops
+    for dtype, tname in ((torch.bfloat16, "__nv_bfloat16"), (torch.float16, "__half")):
+        for seq in (63, 129):
+            qkv = torch.randn(2 * seq, 3 * 128, device="cuda").to(dtype)
+            out = torch.empty(2 * seq, 128, device="cuda", dtype=dtype)
+            kw = dict(D=128, heads=2, group_dims=[2], group_strides=[seq], seq=seq)
+            for causal in (True, False):
+                bias = None if causal else torch.zeros(2, seq, seq, device="cuda")
+                for tc in (-1, 0, 2):
+                    lib.set_option("attn_tc", tc)
+                    try:
+                        got = _attn_launched(lambda: ops.attention(qkv, out, causal=causal, bias=bias, **kw))
+                    finally:
+                        lib.set_option("attn_tc", -1)
+                    want = [(tname, False, False, causal, not causal)]
+                    assert got == want, ((dtype, seq, causal, tc), got, want)
+
+
+@pytest.mark.gpu
+def test_text_attention_refusals():
+    from opendwm_b200 import ops
+    qkv = torch.zeros(2 * 77, 3 * 128, device="cuda", dtype=torch.bfloat16)
+    out = torch.empty(2 * 77, 128, device="cuda", dtype=torch.bfloat16)
+    bias = torch.zeros(2, 77, 77, device="cuda")
+    kw = dict(D=128, heads=2, group_dims=[2], group_strides=[77], seq=77)
+    with pytest.raises(RuntimeError, match="one of causal and bias"):
+        ops.attention(qkv, out, causal=True, bias=bias, **kw)
+    with pytest.raises(RuntimeError, match="contiguous sequences"):   # padded groups
+        ops.attention(torch.zeros(2 * 80, 3 * 128, device="cuda", dtype=torch.bfloat16), out,
+                      causal=True, **dict(kw, group_strides=[80]))
+    with pytest.raises(RuntimeError, match="contiguous sequences"):   # gathered units
+        ops.attention(qkv, out, causal=True, **dict(kw, inner=7, stride_outer=7))
+    with pytest.raises(ValueError, match="bias must be"):
+        ops.attention(qkv, out, bias=bias[:, :76], **kw)

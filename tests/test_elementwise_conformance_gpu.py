@@ -1,6 +1,6 @@
 """Element-wise conformance of the scheduler updates and pixel kernels of rowops.cu / vae.cu
 against float64: cfg_ddim_step, euler_step_by_indices, cfg_euler_step, lincomb2, axpy,
-softmax_rows, act_cast, sinusoid, patchify and upsample_nearest.
+softmax_rows, act_cast, sinusoid, patchify, upsample_nearest and the text encoders' embed.
 
 Bounds.  The arithmetic kernels are restated as float64 expressions over `Fe` values, which carry
 a first-order bound on the fp32 kernel's error: every fp32 operation rounds once (U32 = 2^-24 of
@@ -16,7 +16,8 @@ sinf / cosf (sinusoid) 2 ulps each, with the timestep times the frequency rounde
 exact; the sum of c exponentials in a 256-thread, 8-warp tree adds (ceil(c / 256) + 13) U32
 relative error.  Results below 2^-120 (softmax rows whose scaled range underflows exp2f,
 gelu_tanh where __fdividef flushes to 0) are held to that absolute floor.  patchify and upsample_nearest move values
-and round once: bit-exact against torch.
+and round once: bit-exact against torch.  embed gathers fp32 rows and adds the position row with
+one fp32 addition: bit-exact against torch.nn.functional.embedding (+ pos).
 
 Every deterministic kernel is called twice and must repeat its bits.  groupnorm_stats (atomics)
 is not here: see test_norm_conformance_gpu.
@@ -473,3 +474,52 @@ def test_upsample_nearest_bit_exact(T, compress, C, dtype):
     assert torch.equal(ops.upsample_nearest(xd, compress, dtype), out)
     with pytest.raises(ValueError):
         ops.upsample_nearest(xd.transpose(2, 3), compress, dtype)
+
+
+# --------------------------------------------------------------------------------------------
+# embed (bit-exact)
+# --------------------------------------------------------------------------------------------
+SENT32 = 0x7FABCDEF
+EMBED_GUARD = 3
+EMBED_CASES = [
+    # (D, seq, M, pos): D on both sides of the 128 / 256-thread switch at D = 1024; M not a
+    # multiple of seq (the C API allows a partial last sequence)
+    (4, 5, 23, True),
+    (1020, 77, 251, True),
+    (1024, 77, 251, True),
+    (1284, 77, 160, True),
+    (4096, 77, 100, False),
+    (4096, 16, 50, True),
+]
+
+
+@pytest.mark.parametrize("D,seq,M,pos", EMBED_CASES, ids=["D%d_seq%d_M%d_pos%d" % c for c in EMBED_CASES])
+def test_embed_bit_exact(D, seq, M, pos):
+    """ids 0 and vocab - 1 among random ones; the table inside a NaN / +-Inf allocation; pos
+    [seq + 3, D] whose rows past seq are NaN (the kernel must not read them); the output rows
+    with a pitch of D + 8 inside sentinel guard rows.  Out-of-range ids trap by design and are
+    not called here."""
+    from opendwm_b200 import ops
+    g = _g(D + seq + M)
+    vocab = 1000
+    tok = torch.randn(vocab, D, generator=g)
+    ids = torch.randint(0, vocab, (M,), generator=g)
+    ids[0], ids[M // 2], ids[-1] = vocab - 1, 0, vocab - 1
+    p = torch.cat([torch.randn(seq, D, generator=g), torch.full((3, D), float("nan"))]) if pos else None
+    want = torch.nn.functional.embedding(ids, tok)
+    if pos:
+        want = want + p[torch.arange(M) % seq]
+    tokd, posd, idsd = in_poison(tok), None if p is None else in_block(p), ids.cuda()
+
+    def run():
+        buf = torch.full((M + 2 * EMBED_GUARD, D + 8), SENT32, dtype=torch.int32, device="cuda")
+        ops.embed(idsd, tokd, buf[EMBED_GUARD:-EMBED_GUARD, :D].view(torch.float32), pos=posd, seq=seq)
+        torch.cuda.synchronize()
+        return buf
+
+    buf = run()
+    inside = torch.zeros(buf.shape, dtype=torch.bool, device="cuda")
+    inside[EMBED_GUARD:-EMBED_GUARD, :D] = True
+    assert (buf[~inside] == SENT32).all(), "wrote outside the [M, D] rows"
+    assert torch.equal(buf[EMBED_GUARD:-EMBED_GUARD, :D].cpu(), want.view(torch.int32))
+    assert torch.equal(run(), buf), "the repeated call gave other bits"

@@ -21,11 +21,12 @@ halo-row convolution.  Every GPU case therefore:
     tap order) is held to the bound.  The default call is repeated and must repeat its bits.
     `test_kernel_selection` checks with torch.profiler that the rules pick the launched kernel.
 
-The CPU self-test checks the bound itself against an emulated kernel and seven wrong ones.
+The CPU self-test checks the bound itself against an emulated kernel and ten wrong ones.
 
 Worst ratio |out - ref| / tol over this file's cases, measured on an H100 80GB HBM3 at a 700 W
 power limit (bf16 / fp16): linear 16-bit and F32 0.995 / 0.996, linear RESID 0.909 / 0.909,
-per-tap convolution 0.955 / 0.942, halo-row convolution 0.684 / 0.934.  These maxima sit in
+per-tap convolution 0.955 / 0.942, halo-row convolution 0.684 / 0.934; the text encoders'
+QuickGELU STORE 0.994 / 0.988 and GEGLU_TANH 0.992 / 0.990 (same card, same limit).  These maxima sit in
 the one-rounding terms (the 16-bit output, the fp32 fma of a residual far larger than the
 product), which are exact.  Where the accumulation term dominates, fp32 outputs of sums of
 K = 648 to 2880 products, the error is 0.2 to 0.8 % of acc_bound: the model's linear growth
@@ -42,8 +43,10 @@ import torch
 from opendwm_b200 import lib
 
 STORE, GEGLU, QKNORM, RESID, F32 = lib.EPI_STORE, lib.EPI_GEGLU, lib.EPI_QKNORM, lib.EPI_RESID, lib.EPI_F32
-NONE, GELU_TANH, GELU_ERF, SILU, RELU = (lib.ACT_NONE, lib.ACT_GELU_TANH, lib.ACT_GELU_ERF,
-                                         lib.ACT_SILU, lib.ACT_RELU)
+GEGLU_TANH = lib.EPI_GEGLU_TANH
+NONE, GELU_TANH, GELU_ERF, SILU, RELU, QUICK_GELU = (lib.ACT_NONE, lib.ACT_GELU_TANH, lib.ACT_GELU_ERF,
+                                                     lib.ACT_SILU, lib.ACT_RELU, lib.ACT_QUICK_GELU)
+EPI_STORE_QUICK_GELU = 16  # gemm_epilogue.cuh: the EPI template argument of STORE with act = QUICK_GELU
 SENT16 = -21555          # int16 0xABCD: bits of every 16-bit element the call must not write
 SENT32 = 0x7FABCDEF      # int32 bits of every fp32 element the call must not write (a NaN)
 GUARD = 3                # sentinel rows before and after each output buffer
@@ -87,7 +90,8 @@ def acc_bound(P, K):
     return C_ACC * 2.0 ** -23 * math.ceil(K / K_GRP) * P
 
 
-LIPSCHITZ = {NONE: 1.0, RELU: 1.0, GELU_TANH: 1.13, GELU_ERF: 1.13, SILU: 1.1}
+# QuickGELU's derivative is SiLU's at u = 1.702 x, times 1.702 x / u = 1: the same constant
+LIPSCHITZ = {NONE: 1.0, RELU: 1.0, GELU_TANH: 1.13, GELU_ERF: 1.13, SILU: 1.1, QUICK_GELU: 1.1}
 
 
 def act_reference(x, act):
@@ -95,6 +99,10 @@ def act_reference(x, act):
     gelu_tanh = x / (1 + __expf(-u2)) (__fdividef) and silu = x / (1 + __expf(-x)): __expf is
     accurate to (2 + 1.2 |u2|) ulps and the rounded u2 adds ~4 ulps of |u2|, which moves the
     result by (1 - sigmoid(u2)) times that relative error; the division and 1 + e add 2^-21.
+    quick_gelu = x / (1 + __expf(-1.702f * x)) (gemm_epilogue.cuh, built without fast math: the
+    division is IEEE) is silu's formula at u2 = 1.702 x: the constant 1.702f and the rounded
+    product -1.702f * x move u2 by at most 2 ulps of |u2|, inside the 4 above, so it takes
+    silu's bound with that u2.
     gelu_erf = 0.5 x (1 + erff(x / sqrt2)): erff is within 2 ulps, so 1 + erff has an absolute
     error below 2^-22, times |x| / 2."""
     zero = torch.zeros_like(x)
@@ -105,7 +113,12 @@ def act_reference(x, act):
     if act == GELU_ERF:
         y = 0.5 * x * (1 + torch.erf(x / math.sqrt(2)))
         return y, 2.0 ** -22 * (x.abs() + y.abs())
-    u2 = x if act == SILU else 2 * 0.7978845608028654 * (x + 0.044715 * x ** 3)
+    if act == SILU:
+        u2 = x
+    elif act == QUICK_GELU:
+        u2 = 1.702 * x
+    else:
+        u2 = 2 * 0.7978845608028654 * (x + 0.044715 * x ** 3)
     s = torch.sigmoid(u2)
     y = x * s
     return y, y.abs() * (2.0 ** -21 + (2.0 ** -22 + 2.0 ** -20 * u2.abs()) * (1 - s))
@@ -127,10 +140,14 @@ class Epi:
 
     @property
     def out16(self):
-        return self.kind in (STORE, GEGLU, QKNORM)
+        return self.kind in (STORE, GEGLU, QKNORM, GEGLU_TANH)
+
+    @property
+    def gated(self):
+        return self.kind in (GEGLU, GEGLU_TANH)
 
     def out_cols(self, N):
-        return N // 2 if self.kind == GEGLU else N
+        return N // 2 if self.gated else N
 
     def out_rows(self, M):
         """Output row of each of the M result rows (16-bit outputs are remapped)."""
@@ -187,7 +204,8 @@ def epilogue_reference(z, P, K, e, out_dtype, acc_err=None):
         constant (1.13 for both GELUs, 1.1 for SiLU, 1 for ReLU / none);
       * RESID: v = fma(pre, g, r): |g| E_pre + U32 |v|; blend, fma(a, x, (1 - a) v) with 1 - a
         rounded in fp32: |1 - a| E_v + 2 U32 |(1 - a) v| + U32 |out|;
-      * GEGLU: x * gelu_erf(y): |gelu(y)| E_x + |x| (1.13 E_y + erf error) + U32 |out|;
+      * GEGLU / GEGLU_TANH: x * gelu(y), gelu_erf / gelu_tanh: |gelu(y)| E_x + |x| (1.13 E_y +
+        the activation's own error) + U32 |out|;
       * QKNORM: y = v r w with r = rsqrt(mean(v^2) + eps): to first order |w| r (E_v +
         |v| r max_head E_v) (the perturbation of r is at most r^2 max E_v), plus 2^-18 |y| for
         the fp32 64-term sum of squares (<= 2^-19 relative), rsqrtf and the two products;
@@ -219,10 +237,10 @@ def epilogue_reference(z, P, K, e, out_dtype, acc_err=None):
             y = al * X + a1 * v
             err = a1.abs() * err + 2 * U32 * (a1 * v).abs() + U32 * y.abs()
             floor = floor * a1.abs()
-    elif e.kind == GEGLU:
+    elif e.gated:
         vc, gc = (c.to(z.device) for c in geglu_columns(N))
         x, yg = pre[:, vc], pre[:, gc]
-        ge, e_ge = act_reference(yg, GELU_ERF)
+        ge, e_ge = act_reference(yg, GELU_ERF if e.kind == GEGLU else GELU_TANH)
         y = x * ge
         err = ge.abs() * e_pre[:, vc] + x.abs() * (1.13 * e_pre[:, gc] + e_ge) + U32 * y.abs()
         floor = 2.0 ** -20 * (scale[:, vc] * ge.abs() + x.abs() * scale[:, gc])
@@ -260,6 +278,8 @@ def _fma(a, b, c):
 
 
 def _act32(x, act):
+    if act == QUICK_GELU:
+        return x * torch.sigmoid(1.702 * x)
     if act == GELU_TANH:
         return x * torch.sigmoid(2 * 0.7978845608028654 * (x + 0.044715 * x * x * x))
     if act == GELU_ERF:
@@ -295,18 +315,20 @@ def emulate_epilogue(pre, e, out_dtype, bug=None):
     output type."""
     M, N = pre.shape
     if e.kind in (STORE, F32):
-        y = _act32(pre, e.act)
+        act = SILU if bug == "sigmoid(x) for sigmoid(1.702 x)" else e.act
+        y = _act32(pre, act)
     elif e.kind == RESID:
         R, G, X, al = e.operands(M, bug)
         y = _fma(pre, G if G is not None else torch.ones_like(pre), R if R is not None else torch.zeros_like(pre))
         if X is not None:
             a_ = al.float()
             y = _fma(a_, X, (1 - a_) * y)
-    elif e.kind == GEGLU:
+    elif e.gated:
         vc, gc = geglu_columns(N)
         if bug == "GEGLU halves swapped":
             vc, gc = gc, vc
-        y = pre[:, vc] * torch.nn.functional.gelu(pre[:, gc])
+        tanh = e.kind == GEGLU_TANH and bug != "erf GELU on the gate"
+        y = pre[:, vc] * _act32(pre[:, gc], GELU_TANH if tanh else GELU_ERF)
     else:
         y = pre.clone()
         for h in range(N // 64):
@@ -362,6 +384,8 @@ def _selftest_specs():
         ("QKNORM", 192, Epi(QKNORM, bias=rn(192), qw=rn(64) * 0.2 + 1, kw=rn(64) * 0.2 + 1,
                             qk_region=64), ["RMS over 63 columns"]),
         ("GEGLU", 256, Epi(GEGLU, bias=rn(256)), ["GEGLU halves swapped"]),
+        ("STORE quick_gelu", 96, Epi(STORE, QUICK_GELU, bias=rn(96)), ["sigmoid(x) for sigmoid(1.702 x)"]),
+        ("GEGLU_TANH", 256, Epi(GEGLU_TANH, bias=rn(256)), ["GEGLU halves swapped", "erf GELU on the gate"]),
     ]
 
 
@@ -389,7 +413,7 @@ def test_bound_accepts_emulated_kernel_and_rejects_wrong_ones(dtype):
 # kernel selection, restated from gemm.cu / conv.cu
 # --------------------------------------------------------------------------------------------
 def pick_tile_n(M, N, kind, cl, sms, gemm_bn=0):
-    if kind == GEGLU:
+    if kind in (GEGLU, GEGLU_TANH):
         return 256
     if gemm_bn in (128, 256):
         return gemm_bn
@@ -572,12 +596,33 @@ LINEAR_CASES = [
     _lin("qknorm_joint_context_M90_N960_K72", 90, 960, 72, QKNORM, "NT128_CL1", bias=True,
          qk_region=320, regions=2, rows_per_item=30, out_item_stride=130, out_row_offset=100,
          out_total=390),
+    # text encoders.  CLIP-L's fc1 for one prompt of 77 tokens, and for 12 (a CFG window's
+    # distinct prompts)
+    _lin("store_quick_gelu_M77_N3072_K768", 77, 3072, 768, STORE, "NT128_CL1", act=QUICK_GELU,
+         bias=True),
+    _lin("store_quick_gelu_M924_N3072_K768", 924, 3072, 768, STORE, "NT256_CL2", act=QUICK_GELU,
+         bias=True),
+    _lin("store_quick_gelu_remap_M301_N352_K72", 301, 352, 72, STORE, "NT128_CL1", act=QUICK_GELU,
+         bias=True, rows_per_item=77, out_item_stride=90, out_row_offset=4),
+    # T5's gated tanh-GELU (always 256 wide)
+    _lin("geglu_tanh_nobias_M77_N512_K256", 77, 512, 256, GEGLU_TANH, "NT256_CL1"),
+    _lin("geglu_tanh_M616_N1536_K1024", 616, 1536, 1024, GEGLU_TANH, "NT256_CL2", bias=True),
+    _lin("geglu_tanh_remap_M300_N768_K72", 300, 768, 72, GEGLU_TANH, "NT256_CL1", bias=True,
+         rows_per_item=100, out_item_stride=110, out_row_offset=3),
 ]
 
 
+def _family(kind, act):
+    """The BOUND_RATIO family of a linear case."""
+    if kind == RESID:
+        return "linear_resid"
+    if kind == GEGLU_TANH:
+        return "linear_geglu_tanh"
+    return "linear_quick_gelu" if act == QUICK_GELU else "linear"
+
+
 def _linear_inputs(M, N, K, kind, opt, dtype):
-    out16 = kind in (STORE, GEGLU, QKNORM)
-    a, w = make_operands(M, N, K, dtype, big_scale(dtype, out16), seed=M * 7 + N + K)
+    a, w = make_operands(M, N, K, dtype, big_scale(dtype, Epi(kind).out16), seed=M * 7 + N + K)
     g = torch.Generator().manual_seed(M + N + K)
     rn = lambda *s: torch.randn(*s, generator=g)  # noqa: E731
     rpi = opt.get("rows_per_item", 0)
@@ -671,7 +716,7 @@ def test_linear_conforms(name, shape, label, dtype):
                     "%s gave other bits than %s" % (_label(k), label)
     if kind == RESID:
         assert same(_launch_linear(A, W, e, opt, dtype, resid_tma=0)), "resid_tma = 0 gave other bits"
-    _record("linear_resid" if kind == RESID else "linear", "%s_%s" % (name, dtype), worst)
+    _record(_family(kind, opt.get("act", NONE)), "%s_%s" % (name, dtype), worst)
 
 
 # --------------------------------------------------------------------------------------------
@@ -793,9 +838,10 @@ def test_conv_conforms(name, shape, label, dtype):
 # --------------------------------------------------------------------------------------------
 # which kernel ran
 # --------------------------------------------------------------------------------------------
-def _launched(fn, types=False):
-    """Template arguments of every gemm / conv wgmma kernel `fn` launches, in order; with
-    `types`, each entry ends with the operand and 16-bit output type names (TA, T)."""
+def _launched(fn, types=False, epi=False):
+    """Template arguments of every gemm / conv wgmma kernel `fn` launches, in order; with `epi`,
+    each gemm entry also carries its EPI template argument; with `types`, each entry ends with
+    the operand and 16-bit output type names (TA, T)."""
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         fn()
@@ -807,7 +853,7 @@ def _launched(fn, types=False):
             continue
         args = [re.sub(r"^\((int|bool)\)", "", s.strip()) for s in m.group(2).split(",")]
         if m.group(1) == "gemm":
-            k = (int(args[3]), int(args[4]))
+            k = (int(args[3]), int(args[4])) + ((int(args[2]),) if epi else ())
         else:
             k = (int(args[3]), int(args[4]), args[5] in ("true", "1"))
         found.append(k + tuple(a.split("::")[-1] for a in args[:2]) if types else k)
@@ -830,7 +876,9 @@ def _selection_shapes(sms):
     """Linear (M, N, kind) and conv (nb, t_out, h, w, c_out, kernel) shapes on both sides of each
     threshold: M = 512 for pairs; a shape whose 128-wide tiles save a tenth of the waves and one
     where they do not; C_out 32 / 96 / 320 / 384 / 512; the halo rule's kw, W and segment count;
-    the conv pair rule's 2 x SMs pixel tiles."""
+    the conv pair rule's 2 x SMs pixel tiles.  Then the text encoders' 16-bit-only linears
+    (M, N, kind, act): QuickGELU on both sides of the M = 512 and NT128 / NT256 thresholds
+    (CLIP-L's fc1 for 12 prompts is the NT256_CL2 one), and GEGLU_TANH on both sides of M = 512."""
     lin = [(511, 288, STORE), (512, 288, STORE), (4096, 1536, RESID), (2048, 1536, RESID),
            (2048, 1536, GEGLU), (513, 6144, F32), (1, 64, QKNORM)]
     conv = [(1, 1, 4, 14, c, (1, 3, 3)) for c in (32, 96, 320, 384, 512)]
@@ -839,7 +887,10 @@ def _selection_shapes(sms):
              (1, 1, 2 * sms - 1, 128, 128, (1, 1, 1)), (1, 1, 2 * sms, 128, 128, (1, 1, 1)),
              (1, 1, 2 * sms, 128, 256, (1, 3, 3)), (1, 1, sms, 128, 32, (1, 3, 3)),
              (1, 1, cdiv(sms, 5), 128, 320, (1, 3, 3))]
-    return lin, conv
+    text = [(511, 288, STORE, QUICK_GELU), (512, 288, STORE, QUICK_GELU),
+            (511, 6144, STORE, QUICK_GELU), (924, 3072, STORE, QUICK_GELU),
+            (511, 512, GEGLU_TANH, NONE), (512, 512, GEGLU_TANH, NONE)]
+    return lin, conv, text
 
 
 @pytest.mark.gpu
@@ -848,14 +899,43 @@ def test_kernel_selection():
     run_isolated("test_gemm_conformance_gpu", "check_kernel_selection")
 
 
+def _epi_arg(kind, act):
+    """The EPI template argument dwm_b200_linear instantiates for (epilogue, act)."""
+    return EPI_STORE_QUICK_GELU if kind == STORE and act == QUICK_GELU else kind
+
+
 def check_kernel_selection():
-    """The launched kernel's template arguments (NT, CL; CBN, CL, HALO) are the ones
-    linear_kernel / conv_kernel predict, on both sides of each threshold, for every option
-    setting the conformance cases use; and every kernel named in a case label is among them."""
+    """The launched kernel's template arguments (NT, CL, EPI; CBN, CL, HALO) are the ones
+    linear_kernel / conv_kernel / _epi_arg predict, on both sides of each threshold, for every
+    option setting the conformance cases use; and every kernel named in a case label is among
+    them.  QuickGELU must reach its own instantiation (EPI 16): the generic STORE kernel's
+    run-time activation switch has no QuickGELU branch."""
     from opendwm_b200 import ops
     sms = _sms()
-    lin, conv = _selection_shapes(sms)
+    lin, conv, text = _selection_shapes(sms)
     seen = set()
+    seen_text = set()
+    for M, N, kind, act in text:
+        for dt in (torch.bfloat16, torch.float16):
+            a = torch.randn(M, 64, device="cuda").to(dt)
+            w = torch.randn(N, 64, device="cuda").to(dt)
+            for two in (1, 0):
+                for bn in (0, 128, 256):
+                    want = linear_kernel(M, N, kind, sms, two, bn) + (_epi_arg(kind, act),)
+                    with _Options(gemm_2cta=two, gemm_bn=bn):
+                        got = _launched(lambda: ops.linear(a, w, epilogue=kind, act=act), epi=True)
+                    assert got == [want], ((M, N, kind, act, dt, two, bn), got, want)
+                    seen_text.add((_label(want[:2]), want[2], dt))
+                    seen.add(_label(want[:2]))
+    for dt in (torch.bfloat16, torch.float16):
+        want = {("NT%d_CL%d" % (nt, cl), EPI_STORE_QUICK_GELU, dt) for nt in (128, 256) for cl in (1, 2)}
+        want |= {("NT256_CL%d" % cl, GEGLU_TANH, dt) for cl in (1, 2)}
+        assert want <= seen_text, want - seen_text
+    if sms == H100_SMS:
+        named = {(c[2], _epi_arg(c[1][3], c[1][4].get("act", NONE)), dt) for c in LINEAR_CASES
+                 for dt in (torch.bfloat16, torch.float16)
+                 if c[1][3] == GEGLU_TANH or c[1][4].get("act") == QUICK_GELU}
+        assert named <= seen_text, named - seen_text
     for M, N, kind in lin:
         a = torch.randn(M, 64, device="cuda").bfloat16()
         w = torch.randn(N, 64, device="cuda").bfloat16()
@@ -868,8 +948,8 @@ def check_kernel_selection():
             for bn in (0, 128, 256):
                 want = linear_kernel(M, N, kind, sms, two, bn)
                 with _Options(gemm_2cta=two, gemm_bn=bn):
-                    got = _launched(lambda: ops.linear(a, w, epilogue=kind, **kw))
-                assert got == [want], ((M, N, kind, two, bn), got, want)
+                    got = _launched(lambda: ops.linear(a, w, epilogue=kind, **kw), epi=True)
+                assert got == [want + (kind,)], ((M, N, kind, two, bn), got, want)
                 seen.add(_label(want))
     for nb, t_out, h, w_, c_out, kernel in conv:
         x = torch.randn(nb, t_out + kernel[0] - 1, h, w_, 64, device="cuda").bfloat16()
@@ -943,3 +1023,41 @@ def test_conv_store_with_resid_raises():
     with pytest.raises((ValueError, RuntimeError)):
         ops.conv(x, wt, kernel=(1, 3, 3), epilogue=lib.EPI_STORE, resid=torch.zeros(3, 64, device="cuda"),
                  resid_rows_per_item=56)
+
+
+@pytest.mark.gpu
+def test_text_epilogue_refusals():
+    """QuickGELU exists only as a STORE epilogue and GEGLU_TANH needs the 256-column packing;
+    both are compiled for 16-bit operands only, so E4M3 operands are refused with either."""
+    from opendwm_b200 import ops
+    a = torch.zeros(64, 64, device="cuda", dtype=torch.bfloat16)
+    w = torch.zeros(256, 64, device="cuda", dtype=torch.bfloat16)
+    for epi in (F32, RESID, GEGLU, QKNORM):
+        with pytest.raises(RuntimeError, match="QUICK_GELU needs the DWM_EPI_STORE"):
+            kw = dict(resid=torch.zeros(64, 256, device="cuda")) if epi == RESID else {}
+            if epi == QKNORM:
+                kw = dict(q_norm_weight=torch.ones(64, device="cuda"), qk_region=256, qk_norm_regions=1)
+            ops.linear(a, w, act=QUICK_GELU, epilogue=epi, **kw)
+    for n in (128, 384):
+        with pytest.raises(RuntimeError, match="GEGLU needs N"):
+            ops.linear(a, torch.zeros(n, 64, device="cuda", dtype=torch.bfloat16), epilogue=GEGLU_TANH)
+    f8 = torch.float8_e4m3fn
+    sc = dict(a_scale=torch.ones(64, device="cuda"), w_scale=torch.ones(256, device="cuda"))
+    for kw in (dict(act=QUICK_GELU), dict(epilogue=GEGLU_TANH)):
+        for od in (torch.bfloat16, torch.float16):
+            with pytest.raises(RuntimeError, match="need 16-bit operands"):
+                ops.linear(a.to(f8), w.to(f8), out_dtype=od, **sc, **kw)
+
+
+def test_pack_geglu_matches_geglu_columns():
+    """ops.pack_geglu puts value row j and gate row j of cat([value, gate]) at the accumulator
+    columns geglu_columns(2F) gives output column j (the layout the references assume), with
+    the bias packed alike; T5 packs cat([wi_1, wi_0]) that way."""
+    from opendwm_b200 import ops
+    F = 384
+    w = torch.arange(2 * F, dtype=torch.float32)[:, None].repeat(1, 8)
+    b = torch.arange(2 * F, dtype=torch.float32) + 0.5
+    wp, bp = ops.pack_geglu(w, b)
+    vc, gc = geglu_columns(2 * F)
+    assert torch.equal(wp[vc], w[:F]) and torch.equal(wp[gc], w[F:])
+    assert torch.equal(bp[vc], b[:F]) and torch.equal(bp[gc], b[F:])

@@ -1,5 +1,5 @@
 """Element-wise conformance of the GroupNorm / SpatialNorm kernels (vae.cu), the LayerNorm / AdaLN
-kernels and the E4M3 row quantizer (rowops.cu) against float64.
+kernels, the RMSNorm of the T5 encoder and the E4M3 row quantizer (rowops.cu) against float64.
 
 Every GPU case writes into a sentinel-filled allocation (guard elements before and after, a row
 pitch or frames the call must not touch) and reads inputs whose padding holds NaN / +-Inf.  The
@@ -30,6 +30,14 @@ kernel's arithmetic, each fp32 step rounding by at most U32 = 2^-24 of its resul
     term sums to zero): relative error (4 ceil(D / 128) + 10) U32 + E_mean^2 / var; rstd as
     above.  Each later step (x weight, + bias, x (1 + scale), + shift) adds |factor| E plus
     U32 of its result (and of 1 + scale's rounding).
+  * RMSNorm (`rms_reference`): the sum of squares is fp32, per-thread float4 partials over the
+    row's D / 4 vectors in steps of 256 threads, a 5-level warp shuffle tree and a sequential
+    sum of the 8 warps' partials.  Every term is non-negative, so the sum's relative error is at
+    most L U32 with L = 4 + ceil(D / 1024) + 5 + 7 the longest chain of roundings a square takes
+    part in; / D and + eps add 2 U32, rsqrtf 2 ulps (4 U32) and halves the rest:
+    e_r = (L + 2) U32 / 2 + 4 U32.  out = w (x r), two rounded products: E = (e_r + 2 U32) |ref|.
+    An all-zero row must give 0; fp16 results past 65504 must be +-Inf where the bound puts the
+    exact value beyond fp16's rounding threshold 65520 (and +-65504 or +-Inf within it).
   * E4M3 outputs (GroupNorm: one scale per volume, LayerNorm: per row): amax is the max of the
     kernel's fp32 values, so |448 scale - amax_ref| <= max E + 2^-23 amax_ref.  Each byte's
     fp32 pre-image v * fl(448 / amax) lies within E_p = 448 (E + |ref| E_max / amax_lo) /
@@ -39,16 +47,18 @@ kernel's arithmetic, each fp32 step rounding by at most U32 = 2^-24 of its resul
     all-zero volume or row must give scale 1 and zero bytes.
   * `quantize_rows` is bit-exact against tests/fp8_emulation.quantize_rows.
 
-The CPU self-test runs fp32 emulations of the kernels through the same checks and rejects seven
+The CPU self-test runs fp32 emulations of the kernels through the same checks and rejects nine
 wrong kernels: a one-pass fp32 LayerNorm variance, a GroupNorm group index one channel off for
 10-channel groups, t * Tz / T as the frame map for odd T, eps added outside the square root, the
-modulation of item + 1, an inverted E4M3 scale, and fp32 GroupNorm statistics whose negative
-variance is not clamped.
+modulation of item + 1, an inverted E4M3 scale, fp32 GroupNorm statistics whose negative
+variance is not clamped, and an RMSNorm whose mean runs over D - 4 columns or whose eps sits
+outside the rsqrt.
 
 Worst ratio |out - ref| / tol over this file's cases, measured on an H100 80GB HBM3 at a 700 W
 power limit (bf16 / fp16): groupnorm_stats 0.078; spatialnorm_silu 0.995 / 0.996;
 groupnorm_silu_halo 0.986 / 0.976; layernorm 0.996 / 0.997.  E4M3 scales: groupnorm_silu_e4m3
-0.001, the halo variant 0.020, layernorm 0.136 (every byte within its allowed codes).  The
+0.001, the halo variant 0.020, layernorm 0.136 (every byte within its allowed codes).  rmsnorm
+(bf16 / fp16 / fp32) 0.996 / 0.997 / 0.268, same card and limit.  The
 16-bit maxima sit in the output rounding, which is exact; the statistics use 8 % of a bound that
 assumes every rounding of a double chain as long as the group is adds up.  At the parent
 revision (fp32 statistics) every groupnorm_stats case missed its bound by 3e2 to 4e7 times, and
@@ -864,3 +874,129 @@ def test_quantize_rows_bit_exact(K, dtype):
     mask[GUARD:GUARD + M * ldo].view(M, ldo)[:, :K] = False
     assert not ((buf != SENT8) & mask).any(), "wrote outside [M, K]"
     assert (q_ref[2].float().abs() < 2.0 ** -6).sum() > K // 2
+
+
+# --------------------------------------------------------------------------------------------
+# RMSNorm (T5LayerNorm)
+# --------------------------------------------------------------------------------------------
+SENT32 = 0x7FABCDEF              # int32 bits of every fp32 element a call must not write (a NaN)
+RMS_THREADS = 256
+FP16_MAX, FP16_OVERFLOW = 65504.0, 65520.0   # fp16's largest finite value; RN rounds >= 65520 to Inf
+
+
+def rms_rows(M, D, seed):
+    """[M, D] rows cycling through: benign (0.5 + 2 N(0, 1)); all zero; N(0, 1) scaled by 1e-4
+    (mean square far below eps) and by 1e4; and rows sized like T5-v1.1's residual stream
+    (std 30 with every 331st column 300 times larger)."""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(M, D, generator=g)
+    kind = torch.arange(M) % 5
+    x[kind == 0] = 0.5 + 2 * x[kind == 0]
+    x[kind == 1] = 0
+    x[kind == 2] *= 1e-4
+    x[kind == 3] *= 1e4
+    t5 = x[kind == 4] * 30
+    t5[:, ::331] *= 300
+    x[kind == 4] = t5
+    return x
+
+
+def rms_weight(D, seed, big=True):
+    """1 + 0.2 N(0, 1); with `big`, every 97th entry +-3e5 (fp16 overflows there)."""
+    g = torch.Generator().manual_seed(seed + 1)
+    w = 1 + 0.2 * torch.randn(D, generator=g)
+    if big:
+        w[::97] = 3e5 * (torch.randint(0, 2, w[::97].shape, generator=g) * 2 - 1)
+    return w
+
+
+def rms_reference(x, w, eps):
+    """float64 (ref, err) of w x rsqrt(mean(x^2) + eps), err as the module docstring states."""
+    D = x.shape[1]
+    eps = torch.tensor(eps, dtype=torch.float32).item()
+    xd = x.double()
+    ref = w.double() * xd * torch.rsqrt(xd.pow(2).mean(-1, keepdim=True) + eps)
+    L = 4 + math.ceil(D / (4 * RMS_THREADS)) + 5 + 7
+    return ref, ((L + 2) * U32 / 2 + 6 * U32) * ref.abs()
+
+
+def rms_emulate(x, w, eps, bug=None):
+    """fp32 kernel; `bug` makes it a wrong one."""
+    D = x.shape[1]
+    n = D - 4 if bug == "mean over D - 4 columns" else D
+    ms = (x[:, :n] * x[:, :n]).sum(-1, keepdim=True) / n
+    r = 1 / (ms.sqrt() + eps) if bug == "eps outside the rsqrt" else torch.rsqrt(ms + eps)
+    return w * (x * r)
+
+
+def rms_check(out, ref, err, dtype, what):
+    """out (any device) against (ref, err): the bound, and fp16's overflow to +-Inf."""
+    out = out.cpu().double()
+    tol = out16_tol(err, ref, dtype)
+    if dtype == torch.float16:
+        inf = ref.abs() - tol >= FP16_OVERFLOW           # rounds to Inf whatever the kernel's error
+        edge = ~inf & (ref.abs() + tol >= FP16_OVERFLOW)  # may round either way
+        sign = torch.sign(ref)
+        assert torch.equal(out[inf], sign[inf] * math.inf), "%s: fp16 overflow is not +-Inf" % what
+        ok_edge = (out[edge] == sign[edge] * math.inf) | (out[edge] == sign[edge] * FP16_MAX)
+        assert ok_edge.all(), "%s: fp16 result at the overflow threshold is neither +-65504 nor +-Inf" % what
+        fin = ~(inf | edge)
+        return check16(out[fin], ref[fin], tol[fin], what)
+    return check16(out, ref, tol, what)
+
+
+def test_rmsnorm_bound_accepts_emulated_kernel_and_rejects_wrong_ones():
+    """The fp32 emulation passes the bound in every output type (fp16 overflow included); the
+    mean over D - 4 columns and eps outside the rsqrt fail it, at D = 68 in every type and at
+    D = 1028 in fp32."""
+    for D, dtypes in ((68, (torch.bfloat16, torch.float16, torch.float32)), (1028, (torch.float32,))):
+        x, w = rms_rows(40, D, seed=D), rms_weight(D, seed=D)
+        ref, err = rms_reference(x, w, 1e-6)
+        for dtype in dtypes:
+            rms_check(rms_emulate(x, w, 1e-6).to(dtype), ref, err, dtype, "emulated")
+            if dtype == torch.float16:
+                assert (ref.abs() > FP16_OVERFLOW).any(), "the case must overflow fp16"
+            for bug in ("mean over D - 4 columns", "eps outside the rsqrt"):
+                with pytest.raises(AssertionError):
+                    rms_check(rms_emulate(x, w, 1e-6, bug).to(dtype), ref, err, dtype, bug)
+
+
+RMS_CASES = [(1, 4), (77, 1020), (300, 1024), (5, 1028), (77, 1284), (2053, 4096), (300, 4100),
+             (3001, 1024)]
+RMS_LDO_PAD = 12
+
+
+def _rms_launch(xd, wd, dtype):
+    """One call into a fresh sentinel allocation: (flat buffer, [M, D] view of pitch D + 12)."""
+    from opendwm_b200 import ops
+    M, D = xd.shape
+    n = M * (D + RMS_LDO_PAD)
+    if dtype == torch.float32:
+        buf = torch.full((n + 2 * GUARD,), SENT32, dtype=torch.int32, device="cuda")
+    else:
+        buf = torch.full((n + 2 * GUARD,), SENT16, dtype=torch.int16, device="cuda")
+    view = buf[GUARD:GUARD + n].view(dtype).view(M, D + RMS_LDO_PAD)[:, :D]
+    ops.rmsnorm(xd, wd, view, eps=1e-6)
+    torch.cuda.synchronize()
+    return buf, view
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16, torch.float32], ids=["bf16", "fp16", "fp32"])
+@pytest.mark.parametrize("M,D", RMS_CASES, ids=["M%d_D%d" % c for c in RMS_CASES])
+def test_rmsnorm_conforms(M, D, dtype):
+    """x with a NaN / +-Inf row pitch, the weight inside a NaN / +-Inf allocation, the output in
+    a sentinel allocation with a pitch and guard elements.  D = 1020 / 1024 / 1028: both sides
+    of one pass of 256 threads x float4; 4096 / 4100: four passes and a ragged fifth."""
+    x, w = rms_rows(M, D, seed=M + D), rms_weight(D, seed=D)
+    ref, err = rms_reference(x, w, 1e-6)
+    xd, wd = _pitched(x), in_poison(w)
+    buf, out = _rms_launch(xd, wd, dtype)
+    mask = torch.ones(buf.shape, dtype=torch.bool, device="cuda")
+    mask[GUARD:GUARD + M * (D + RMS_LDO_PAD)].view(M, -1)[:, :D] = False
+    sent = SENT32 if dtype == torch.float32 else SENT16
+    assert not ((buf != sent) & mask).any(), "wrote outside the [M, D] rows"
+    assert (out[(torch.arange(M) % 5 == 1).cuda()] == 0).all(), "an all-zero row must give 0"
+    worst = rms_check(out, ref, err, dtype, "rmsnorm_M%d_D%d" % (M, D))
+    assert torch.equal(_rms_launch(xd, wd, dtype)[0], buf), "the repeated call gave other bits"
+    _record("rmsnorm", "M%d_D%d_%s" % (M, D, dtype), worst)
