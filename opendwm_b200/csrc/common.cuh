@@ -43,6 +43,10 @@ void set_last_error(const char* fmt, ...);
 int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols,
                  uint64_t ld, uint32_t box_rows, uint32_t box_cols, int elem_bytes);
 
+// The same for items x rows x cols with item pitch `item_ld` elements; a box is one item deep.
+int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t items, uint64_t rows, uint64_t cols,
+                 uint64_t ld, uint64_t item_ld, uint32_t box_rows, uint32_t box_cols, int elem_bytes);
+
 int make_tmap_nd(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                  const uint64_t* strides_bytes, const uint32_t* box, int elem_bytes);
 
@@ -160,6 +164,31 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint64_t* bar,
       : "r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
         "r"(c2), "r"(c3), "r"(c4), "l"(hint)
       : "memory");
+}
+
+// 3-D box store shared -> global, tracked by this thread's bulk async-groups; the parts of the
+// box outside the tensor map are not written.
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the shared-memory sources of all committed bulk stores of this thread have been read
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// all committed bulk stores of this thread are complete
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// named barrier over `n` threads (barrier 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int n) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+// four 8x8 16-bit matrices to shared memory: lanes 8i..8i+7 give the row addresses of matrix i,
+// register i of lane l holds row l/4, columns 2(l%4), 2(l%4)+1 of matrix i (the mma fragment)
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
 }
 
 // ---- clusters of two CTAs ----------------------------------------------------

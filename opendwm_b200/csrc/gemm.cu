@@ -9,7 +9,10 @@
 //                  runs ahead into the next tile while the consumers drain the current one
 //   warpgroups 1-2 consumers: each issues wgmma m64nNTk16 (k32 for E4M3) for its 64 rows of
 //                  the tile and then applies the fused epilogue straight from its register
-//                  fragment (E4M3: after scaling it by the row and channel scales)
+//                  fragment (E4M3: after scaling it by the row and channel scales); 16-bit
+//                  outputs go to shared memory and leave by TMA store (TmaOut), so the
+//                  warpgroup returns to the next tile's MMAs while the stores drain, except
+//                  when they are also scattered to peer GPUs, which is done from registers
 // A stage is 128 bytes of K per row in either case: 64 16-bit or 128 E4M3 elements.
 // NT = 256 (the widest wgmma; 128 accumulator registers per thread) unless the 256-wide tiles
 // leave most SMs idle (pick_tile_n).
@@ -26,11 +29,14 @@ namespace dwm {
 constexpr int STAGES = 4;
 constexpr int A_STAGE_BYTES = BM * BK * 2;
 
+// The epilogue region holds either the TMA store boxes or the fp32 transpose buffers of the
+// register path: one launch uses one of them.
+static_assert(EPI_BOXES_BYTES >= EPI_STAGE_BYTES, "epilogue region");
 template <int NT>
 struct GemmCfg {
   static constexpr int kBStageBytes = NT * BK * 2;
   static constexpr int kSmemBytes =
-      STAGES * (A_STAGE_BYTES + kBStageBytes) + EPI_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+      STAGES * (A_STAGE_BYTES + kBStageBytes) + EPI_BOXES_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 // CL = 2: a cluster of two CTAs computes two vertically adjacent output tiles that share one
@@ -43,7 +49,8 @@ struct GemmCfg {
 template <typename TA, typename T, int EPI, int NT, int CL>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                      const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
+                      const __grid_constant__ CUtensorMap tmap_b,
+                      const __grid_constant__ CUtensorMap tmap_out, int M, int N, int K,
                       EpiParams p) {
   constexpr int B_STAGE_BYTES = GemmCfg<NT>::kBStageBytes;
   constexpr int BKE = BK * 2 / static_cast<int>(sizeof(TA));   // K elements per stage
@@ -52,8 +59,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + EPI_STAGE_BYTES);
+  uint8_t* epi_region = smem + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES);   // 1024-byte aligned
+  float* epi_stage = reinterpret_cast<float*>(epi_region);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_region + EPI_BOXES_BYTES);
   uint64_t* full_bar = bars;                 // [STAGES]  TMA -> consumers
   uint64_t* empty_bar = bars + STAGES;       // [STAGES]  consumers (of both CTAs when CL = 2) -> TMA
 
@@ -114,6 +122,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     const int cw = wg - 1;                       // 64-row half of the tile
     const int wrow = cw * 64 + (warp & 3) * 16;  // first tile row of this warp
     float* stg = epi_stage + (warp - 4) * 512;
+    TmaOut tout{epi_out16(EPI) && p.tma_out, &tmap_out, epi_region + cw * 2 * EPI_BOX_BYTES, 1 + cw,
+                (threadIdx.x & 127) == 0, 0};
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = first; tile < num_tiles; tile += step) {
@@ -126,8 +136,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                               empty_bar, STAGES, k_blocks, stage, phase, lane, rank ^ 1u);
       if constexpr (sizeof(TA) == 1)
         dequant_frag<NT>(acc, p.a_scale, p.w_scale, m_blk * BM + wrow, M, n_blk * NT, N, lane);
-      drain_tile<T, EPI, NT>(acc, stg, m_blk * BM, wrow, M, n_blk * NT, N, p, lane);
+      drain_tile<T, EPI, NT>(acc, stg, m_blk * BM, wrow, M, n_blk * NT, N, p, lane, TileGeom{0, 0, 0, 0, 0}, &tout);
     }
+    if (tout.on && tout.leader) bulk_wait_all();   // no CTA exits with its stores in flight
   }
   // a CTA of a pair must not exit while its peer may still multicast into it or arrive on it
   if constexpr (CL == 2) cluster_sync_all();
@@ -147,6 +158,24 @@ static int launch_gemm(const dwm_linear_args* a, cudaStream_t stream) {
   EpiParams p;
   fill_epi_params(p, a);
   p.resid_prefetch = g_resid_tma;
+  // 16-bit outputs by TMA store: the whole items [items, rows per item, N] at the remapped rows
+  // (a layout without items is one item of M rows); the rows of a partial last item are copied
+  // by the consumer threads
+  CUtensorMap to = {};
+  if (epi_out16(EPI) && a->n_peer_out == 0) {
+    const long long rpi = a->rows_per_item > 0 ? a->rows_per_item : a->M;
+    const long long items = a->M / rpi;
+    const long long item_ld = (a->rows_per_item > 0 ? a->out_item_stride : a->M) * a->ldo;
+    const long long n_out = (EPI == DWM_EPI_GEGLU || EPI == DWM_EPI_GEGLU_TANH) ? a->N / 2 : a->N;
+    if (items > 0) {
+      rc = make_tmap_3d(&to, reinterpret_cast<const T*>(a->out) + a->out_row_offset * a->ldo, items, rpi, n_out,
+                        a->ldo, item_ld, 64, 64, 2);
+      if (rc) return rc;
+    }
+    p.tma_out = 1;
+    p.out_rpi = static_cast<int>(rpi);
+    p.out_items = static_cast<int>(items);
+  }
 
   constexpr int smem_bytes = GemmCfg<NT>::kSmemBytes;
   auto kern = gemm_wgmma_kernel<TA, T, EPI, NT, CL>;
@@ -162,10 +191,10 @@ static int launch_gemm(const dwm_linear_args* a, cudaStream_t stream) {
   const int grid = CL * static_cast<int>(tiles < slots ? tiles : slots);
   const int Mi = static_cast<int>(a->M), Ni = static_cast<int>(a->N), Ki = static_cast<int>(a->K);
   if constexpr (CL == 1) {
-    kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(ta, tb, Mi, Ni, Ki, p);
+    kern<<<grid, GEMM_THREADS, smem_bytes, stream>>>(ta, tb, to, Mi, Ni, Ki, p);
   } else {
     DWM_CHECK_CUDA(launch_cluster2(kern, grid, GEMM_THREADS, smem_bytes, stream,
-                                   ta, tb, Mi, Ni, Ki, p));
+                                   ta, tb, to, Mi, Ni, Ki, p));
   }
   DWM_CHECK_CUDA(cudaGetLastError());
   return 0;

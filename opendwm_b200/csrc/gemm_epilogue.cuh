@@ -14,12 +14,21 @@ constexpr int CONSUMER_WGS = 2;
 constexpr int GEMM_THREADS = 128 * (1 + CONSUMER_WGS);   // warpgroup 0: TMA producer
 constexpr int EPI_WARPS = 4 * CONSUMER_WGS;
 constexpr int EPI_STAGE_BYTES = EPI_WARPS * 16 * 32 * 4;  // per consumer warp: 16x32 fp32
+// TMA-stored 16-bit outputs: a 64 x 64 box (128B-swizzled, 128 bytes per row), two per warpgroup
+constexpr int EPI_BOX_BYTES = 64 * 64 * 2;
+constexpr int EPI_BOXES_BYTES = CONSUMER_WGS * 2 * EPI_BOX_BYTES;
 // register split (65536 per SM, one CTA): producer warpgroup 40, consumers 232 each
 constexpr int PRODUCER_REGS = 40;
 constexpr int CONSUMER_REGS = 232;
 // DWM_EPI_STORE with act = DWM_ACT_QUICK_GELU, compiled as an epilogue of its own so that the
 // run-time activation switch of DWM_EPI_STORE keeps its instructions
 constexpr int EPI_STORE_QUICK_GELU = 16;
+
+// epilogues whose output is the 16-bit tile (the others read-modify-write fp32)
+__host__ __device__ constexpr bool epi_out16(int epi) {
+  return epi == DWM_EPI_STORE || epi == DWM_EPI_GEGLU || epi == DWM_EPI_QKNORM || epi == EPI_STORE_QUICK_GELU ||
+         epi == DWM_EPI_GEGLU_TANH;
+}
 
 __device__ __forceinline__ float quick_gelu(float x) { return x / (1.0f + __expf(-1.702f * x)); }
 
@@ -47,6 +56,26 @@ struct EpiParams {
   int resid_prefetch;   // RESID: L2 prefetch of the tile's residual / blend rows by the TMA unit
   const float* a_scale;  // FP8 operands: row scales of A [M] and of W [N]
   const float* w_scale;
+  // 16-bit outputs stored by TMA (see TmaOut): the M rows are out_items whole items of out_rpi
+  // rows (a layout without items: one item of M rows), then the rows of a partial last item
+  int tma_out;
+  int out_rpi, out_items;
+};
+
+// A consumer warpgroup's TMA store of its 16-bit tile rows, box by box.  The warps write a
+// 64 x 64 box into one of two swizzled shared-memory buffers with stmatrix; one leader thread
+// stores it through `map`, the whole items [out_items, out_rpi, N] (row pitch ldo, item pitch
+// out_item_stride * ldo, based at the output's first row), and commits it as a bulk
+// async-group.  The store starts at the box's first row, so its coordinates are never negative,
+// and TMA clips it to that row's item and to N.  The rows of the box in later items, or in a
+// partial last item, are copied from the box by the warpgroup's threads.
+struct TmaOut {
+  bool on;          // false: the register path stores the rows
+  const CUtensorMap* map;
+  uint8_t* bufs;    // this warpgroup's two boxes
+  int bar;          // named barrier of this warpgroup
+  bool leader;      // the thread that stores (and owns the bulk async-groups)
+  uint32_t boxes;   // boxes stored so far: the parity picks the buffer
 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -118,13 +147,14 @@ struct TileGeom {
   int img_w;
 };
 
-// acc: the NT-column fragment of this warp's warpgroup; row0: tile row of the warp's first row
+// acc: the NT-column fragment of this warp's warpgroup; row0: tile row of the warp's first row.
+// tma (linear tiles with 16-bit outputs only): store the rows by TMA instead of from registers.
 template <typename T, int EPI, int NT>
 __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* stg, int m_base, int row0, int M,
                                            int n_tile0, int N, const EpiParams& p, int lane,
-                                           const TileGeom geom = TileGeom{0, 0, 0, 0, 0}) {
-  constexpr bool kOut16 = (EPI == DWM_EPI_STORE || EPI == DWM_EPI_GEGLU || EPI == DWM_EPI_QKNORM ||
-                           EPI == EPI_STORE_QUICK_GELU || EPI == DWM_EPI_GEGLU_TANH);
+                                           const TileGeom geom = TileGeom{0, 0, 0, 0, 0}, TmaOut* tma = nullptr) {
+  constexpr bool kOut16 = epi_out16(EPI);
+  const bool use_tma = kOut16 && tma != nullptr && tma->on;
   const int rs = lane >> 3;  // phase-2: row within a group of 4
   const int c4 = lane & 7;   // phase-2: float4 column within the 32-col chunk
 
@@ -135,7 +165,7 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
   float alpha[4];
   const int rpi = static_cast<int>(p.rows_per_item);
 #pragma unroll
-  for (int it = 0; it < 4; ++it) {
+  for (int it = 0; it < 4 && !use_tma; ++it) {
     int m;
     bool valid;
     if (geom.bw > 0) {
@@ -182,6 +212,62 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
         for (int q = 0; q < p.n_peers; ++q)
           *reinterpret_cast<uint2*>(reinterpret_cast<T*>(p.peer_out[q]) + eoff) = pk;
       }
+    }
+  };
+  // TMA path: the 32-column chunk at output column `ocol` goes to its half of the current box
+  // (boxes start at multiples of 64 columns); box_store(ocol) then stores that box
+  auto box_put = [&](const float (&v)[16], int ocol) {
+    const uint32_t buf = smem_u32(tma->bufs + (tma->boxes & 1) * EPI_BOX_BYTES);
+    const int i = lane >> 3;                               // the 8x8 matrix this lane addresses
+    const int r = (row0 & 63) + (i & 1) * 8 + (lane & 7);  // its box row
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {   // n8 blocks 2q and 2q + 1 of the chunk, rows 0-7 and 8-15 each
+      const int c16 = ((ocol >> 5) & 1) * 4 + 2 * q + (i >> 1);   // 16-byte column in the box row
+      stmatrix_x4(buf + r * 128 + ((c16 ^ (r & 7)) << 4), Cvt<T>::pack2(v[8 * q], v[8 * q + 1]),
+                  Cvt<T>::pack2(v[8 * q + 2], v[8 * q + 3]), Cvt<T>::pack2(v[8 * q + 4], v[8 * q + 5]),
+                  Cvt<T>::pack2(v[8 * q + 6], v[8 * q + 7]));
+    }
+  };
+  auto box_store = [&](int ocol) {
+    fence_proxy_async();                       // this thread's stmatrix writes -> the TMA unit
+    if (tma->leader) bulk_wait_read_all();     // the previous box's store has read the other buffer
+    named_bar_sync(tma->bar, 128);
+    const uint8_t* buf = tma->bufs + (tma->boxes & 1) * EPI_BOX_BYTES;
+    const int m0 = m_base + (row0 & ~63), col = ocol & ~63;
+    const int item = m0 / p.out_rpi, r = m0 - item * p.out_rpi;
+    if (tma->leader) {
+      if (item < p.out_items) tma_store_3d(tma->map, buf, col, r, item);
+      bulk_commit();
+    }
+    // rows [j0, j1) of the box are past the end of the stored item (or in a partial last item):
+    // 8 threads per row, 16 bytes each, un-swizzled from the box.  The buffer is rewritten only
+    // after the next box's barrier, which every thread reaches after its copies.
+    const int j0 = item < p.out_items ? p.out_rpi - r : 0;
+    const int j1 = M - m0 < 64 ? M - m0 : 64;
+    if (j0 < j1) {
+      const int t = ((row0 & 63) << 1) + lane;   // thread of the warpgroup
+      const int c = t & 7;
+      const int n_out = (EPI == DWM_EPI_GEGLU || EPI == DWM_EPI_GEGLU_TANH) ? N / 2 : N;
+#pragma unroll 1
+      for (int j = j0 + (t >> 3); j < j1; j += 16) {
+        const int m = m0 + j;
+        if (col + 8 * c < n_out) {
+          const long long o = static_cast<long long>(m / p.out_rpi) * p.out_item_stride + m % p.out_rpi + p.out_row_offset;
+          *reinterpret_cast<uint4*>(reinterpret_cast<T*>(p.out) + o * p.ldo + col + 8 * c) =
+              *reinterpret_cast<const uint4*>(buf + j * 128 + ((c ^ (j & 7)) << 4));
+        }
+      }
+    }
+    ++tma->boxes;
+  };
+  // 16-bit chunk at output column `ocol`; box_done: the last chunk of its box
+  auto put16 = [&](const float (&v)[16], int ocol, bool box_done) {
+    if (use_tma) {
+      box_put(v, ocol);
+      if (box_done) box_store(ocol);
+    } else {
+      stage_dump(stg, lane, v);
+      flush16(ocol);
     }
   };
   // phase 2 for fp32 outputs (optionally gated / residual / blended).  The residual
@@ -263,9 +349,15 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
           for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
         }
       }
-      stage_dump(stg, lane, v);
-      if constexpr (EPI == DWM_EPI_STORE || EPI == EPI_STORE_QUICK_GELU) flush16(n0); else flush32(n0);
+      if constexpr (kOut16) {
+        put16(v, n0, c & 1);
+      } else {
+        stage_dump(stg, lane, v);
+        flush32(n0);
+      }
     }
+    // N % 64 = 32: the last box of the row holds one chunk (one store site, not one per chunk)
+    if (use_tma && N - n_tile0 < NT && ((N - n_tile0) & 32)) box_store(N - 32);
   } else if constexpr (EPI == DWM_EPI_GEGLU || EPI == DWM_EPI_GEGLU_TANH) {
     static_assert(NT == 256, "GEGLU packs value / gate halves per 256-column tile");
     // tile columns [0,128) hold the value half, [128,256) the gate half of output
@@ -286,8 +378,7 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
         }
         v[j] = x * (EPI == DWM_EPI_GEGLU ? gelu_erf(y) : gelu_tanh(y));
       }
-      stage_dump(stg, lane, v);
-      flush16(n_tile0 / 2 + c * 32);
+      put16(v, n_tile0 / 2 + c * 32, c & 1);
     }
   } else {  // DWM_EPI_QKNORM: 64-column heads
 #pragma unroll
@@ -329,10 +420,8 @@ __device__ __forceinline__ void drain_tile(const float (&acc)[NT / 2], float* st
           v1[j] = v1[j] * inv * __ldg(w + 32 + col);
         }
       }
-      stage_dump(stg, lane, v0);
-      flush16(n0);
-      stage_dump(stg, lane, v1);
-      flush16(n0 + 32);
+      put16(v0, n0, false);
+      put16(v1, n0 + 32, true);
     }
   }
 }
@@ -515,6 +604,8 @@ inline void fill_epi_params(EpiParams& p, const dwm_linear_args* a) {
   for (int i = 0; i < 8; ++i) p.peer_out[i] = i < a->n_peer_out ? a->peer_out[i] : nullptr;
   p.a_scale = a->a_scale;
   p.w_scale = a->w_scale;
+  p.tma_out = 0;
+  p.out_rpi = p.out_items = 0;
 }
 
 }  // namespace dwm

@@ -51,11 +51,12 @@ namespace {
 struct TmapKey {
   const void* base;
   uint64_t rows, cols, ld;
+  uint64_t items, item_ld;   // 0, 0 for a 2-D map
   uint32_t box_rows, box_cols;
   int elem;
   bool operator==(const TmapKey& o) const {
-    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows &&
-           box_cols == o.box_cols && elem == o.elem;
+    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && items == o.items &&
+           item_ld == o.item_ld && box_rows == o.box_rows && box_cols == o.box_cols && elem == o.elem;
   }
 };
 struct TmapHash {
@@ -63,6 +64,7 @@ struct TmapHash {
     uint64_t h = reinterpret_cast<uint64_t>(k.base) * 0x9E3779B97F4A7C15ull;
     h ^= (k.rows + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2));
     h ^= (k.cols * 0xC2B2AE3D27D4EB4Full + (h << 6) + (h >> 2));
+    h ^= (k.items * 0x165667B19E3779F9ull + k.item_ld + (h << 6) + (h >> 2));
     h ^= (k.ld + (static_cast<uint64_t>(k.box_rows) << 40) + (static_cast<uint64_t>(k.box_cols) << 20) +
           static_cast<uint64_t>(k.elem) + (h << 6) + (h >> 2));
     return static_cast<size_t>(h);
@@ -72,22 +74,40 @@ std::mutex g_tmap_mu;
 std::unordered_map<TmapKey, CUtensorMap, TmapHash> g_tmap_cache;
 }  // namespace
 
-int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
-                 uint32_t box_rows, uint32_t box_cols, int elem_bytes) {
-  const TmapKey key{base, rows, cols, ld, box_rows, box_cols, elem_bytes};
-  {
-    std::lock_guard<std::mutex> lk(g_tmap_mu);
-    auto it = g_tmap_cache.find(key);
-    if (it != g_tmap_cache.end()) {
-      memcpy(map, &it->second, sizeof(CUtensorMap));
-      return 0;
-    }
-  }
-  const int rc = encode_tmap_2d(map, base, rows, cols, ld, box_rows, box_cols, elem_bytes);
-  if (rc) return rc;
+static bool tmap_cached(const TmapKey& key, CUtensorMap* map) {
+  std::lock_guard<std::mutex> lk(g_tmap_mu);
+  auto it = g_tmap_cache.find(key);
+  if (it == g_tmap_cache.end()) return false;
+  memcpy(map, &it->second, sizeof(CUtensorMap));
+  return true;
+}
+
+static void tmap_cache_put(const TmapKey& key, const CUtensorMap* map) {
   std::lock_guard<std::mutex> lk(g_tmap_mu);
   if (g_tmap_cache.size() > 8192) g_tmap_cache.clear();
   g_tmap_cache.emplace(key, *map);
+}
+
+int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
+                 uint32_t box_rows, uint32_t box_cols, int elem_bytes) {
+  const TmapKey key{base, rows, cols, ld, 0, 0, box_rows, box_cols, elem_bytes};
+  if (tmap_cached(key, map)) return 0;
+  const int rc = encode_tmap_2d(map, base, rows, cols, ld, box_rows, box_cols, elem_bytes);
+  if (rc) return rc;
+  tmap_cache_put(key, map);
+  return 0;
+}
+
+int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t items, uint64_t rows, uint64_t cols,
+                 uint64_t ld, uint64_t item_ld, uint32_t box_rows, uint32_t box_cols, int elem_bytes) {
+  const TmapKey key{base, rows, cols, ld, items, item_ld, box_rows, box_cols, elem_bytes};
+  if (tmap_cached(key, map)) return 0;
+  const uint64_t dims[3] = {cols, rows, items};
+  const uint64_t strides[2] = {ld * static_cast<uint64_t>(elem_bytes), item_ld * static_cast<uint64_t>(elem_bytes)};
+  const uint32_t box[3] = {box_cols, box_rows, 1};
+  const int rc = make_tmap_nd(map, base, 3, dims, strides, box, elem_bytes);
+  if (rc) return rc;
+  tmap_cache_put(key, map);
   return 0;
 }
 

@@ -29,6 +29,9 @@ SHAPES = [
     (86016, 1536, 1536, "resid"), (86016, 1536, 1536, "resid_blend"), (86016, 1536, 1536, "store"),
     (86016, 4608, 1536, "qknorm"), (86016, 6144, 1536, "store"),
     (29568, 4608, 1536, "qknorm"), (29568, 4608, 1536, "store"),
+    # the same projections as the step runs them: into the joint q|k|v buffer, 448 sample rows
+    # then 154 context rows per item, item pitch 602 rows (16-bit stores remapped per item)
+    (86016, 4608, 1536, "qknorm_joint_sample"), (29568, 4608, 1536, "qknorm_joint_context"),
     (29568, 1536, 1536, "resid"), (29568, 1536, 1536, "store"),
     (29568, 6144, 1536, "store"), (29568, 1536, 6144, "resid"), (29568, 1536, 6144, "store"),
     (8192, 8192, 8192, "store"),
@@ -89,10 +92,15 @@ def operands(M, N, K, epi, dtype):
         if epi == "resid_blend":
             kw.update(blend_x=kw["out"], alpha=torch.tensor([0.3, 0.9], device="cuda"),
                       rows_per_batch=M // 2)
-    elif epi == "qknorm":
+    elif epi.startswith("qknorm"):
         qw = torch.ones(64, device="cuda")
         kw.update(epilogue=lib.EPI_QKNORM, q_norm_weight=qw, k_norm_weight=qw, qk_region=N // 3,
                   out=torch.empty(M, N, device="cuda", dtype=dtype))
+        if epi.startswith("qknorm_joint"):
+            S, L = 448, 154
+            rpi = S if epi == "qknorm_joint_sample" else L
+            kw.update(rows_per_item=rpi, out_item_stride=S + L, out_row_offset=0 if rpi == S else S,
+                      out=torch.zeros(M // rpi * (S + L), N, device="cuda", dtype=dtype))
     else:
         kw.update(out=torch.empty(M, N, device="cuda", dtype=dtype))
     return a, w, kw
