@@ -469,6 +469,19 @@ int dwm_b200_upsample_nearest(const float* x, int64_t nb, int64_t T, int64_t H, 
 int dwm_b200_lincomb2(const float* x, const float* y, const float* s0, const float* s1, int64_t n,
                       int64_t inner, float* out, dwm_stream_t stream);
 
+/* Fused CFG combine + DPM-Solver++ step (midpoint, order <= 2) of
+ * src/dwm/schedulers/dpm_solver.py, in place over n fp32 elements:
+ *   m  = w_uncond * u + w_cond * c      (cfg 2: pred = [u ; c], 2n; cfg 1: m = pred, n)
+ *   x0 = c_x * latents + c_m * m
+ *   p  = k_s * latents + k_0 * x0 (+ k_1 * x0_prev when order == 2)
+ *   x0_prev <- x0;  latents <- p
+ * row: fp32 [6] in device memory, (c_x, c_m, k_s, k_0, k_1, order) with order 1 or 2, so that
+ * a captured CUDA graph replays whichever step was loaded into it.  Every line is rounded to
+ * fp32 as dwm_b200_lincomb2 rounds it; a first-order step does not read x0_prev.  latents and
+ * x0_prev must not overlap each other, pred or row. */
+int dwm_b200_cfg_dpmpp_step(const float* pred, int cfg, float w_uncond, float w_cond, int64_t n,
+                            const float* row, float* latents, float* x0_prev, dwm_stream_t stream);
+
 /* y += a * x over n fp32 elements (adapter residual adds of the UNet,
  * crossview_temporal_unet.py:729-731, 759-761). */
 int dwm_b200_axpy(const float* x, float* y, int64_t n, float a, dwm_stream_t stream);

@@ -592,6 +592,31 @@ __global__ void lincomb2_kernel(const float* __restrict__ x, const float* __rest
   out[i] = s0[it] * x[i] + s1[it] * y[i];
 }
 
+// s0 * x + s1 * y rounded as nvcc contracts lincomb2_kernel's expression: fma(s0, x, s1 * y).
+// Spelled out so that a literal s0 = 1 cannot be folded into a different contraction.
+__device__ __forceinline__ float lincomb2_rn(float s0, float x, float s1, float y) {
+  return __fmaf_rn(s0, x, __fmul_rn(s1, y));
+}
+
+// Fused CFG combine + DPM-Solver++ (midpoint, order <= 2) step, in place; the same roundings as
+// the chain of lincomb2 launches it replaces.  row = (c_x, c_m, k_s, k_0, k_1, order) is read
+// from device memory, so a replayed CUDA graph takes the step its caller loaded.  A first-order
+// step never reads x0_prev.
+__global__ void cfg_dpmpp_kernel(const float* __restrict__ pred, int cfg, float w_u, float w_c, long long n,
+                                 const float* __restrict__ row, float* __restrict__ lat,
+                                 float* __restrict__ x0_prev) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float m = pred[i];
+  if (cfg == 2) m = lincomb2_rn(w_u, m, w_c, pred[i + n]);
+  const float x = lat[i];
+  const float x0 = lincomb2_rn(__ldg(row), x, __ldg(row + 1), m);
+  float p = lincomb2_rn(__ldg(row + 2), x, __ldg(row + 3), x0);
+  if (__ldg(row + 5) == 2.f) p = lincomb2_rn(1.f, p, __ldg(row + 4), x0_prev[i]);
+  x0_prev[i] = x0;
+  lat[i] = p;
+}
+
 }  // namespace dwm
 
 using namespace dwm;
@@ -640,6 +665,27 @@ extern "C" int dwm_b200_lincomb2(const float* x, const float* y, const float* s0
   DWM_REQUIRE(x && y && s0 && s1 && out && n > 0 && inner > 0 && n % inner == 0, "dwm_b200_lincomb2: bad arguments");
   const unsigned grid = static_cast<unsigned>((n + 255) / 256);
   lincomb2_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, y, s0, s1, n, inner, out);
+  DWM_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+static bool disjoint(const float* a, int64_t na, const float* b, int64_t nb) {
+  return a + na <= b || b + nb <= a;
+}
+
+extern "C" int dwm_b200_cfg_dpmpp_step(const float* pred, int cfg, float w_uncond, float w_cond, int64_t n,
+                                       const float* row, float* latents, float* x0_prev, dwm_stream_t stream) {
+  DWM_REQUIRE(pred && row && latents && x0_prev, "dwm_b200_cfg_dpmpp_step: null pred/row/latents/x0_prev");
+  DWM_REQUIRE(cfg == 1 || cfg == 2, "dwm_b200_cfg_dpmpp_step: cfg must be 1 or 2, got %d", cfg);
+  DWM_REQUIRE(n > 0 && (n + 255) / 256 <= INT32_MAX, "dwm_b200_cfg_dpmpp_step: bad n %lld", (long long)n);
+  DWM_REQUIRE(is_aligned(pred, 4) && is_aligned(row, 4) && is_aligned(latents, 4) && is_aligned(x0_prev, 4),
+              "dwm_b200_cfg_dpmpp_step: pred, row, latents, x0_prev must be 4-byte aligned");
+  DWM_REQUIRE(disjoint(latents, n, x0_prev, n) && disjoint(latents, n, pred, cfg * n) &&
+                  disjoint(x0_prev, n, pred, cfg * n) && disjoint(row, 6, latents, n) && disjoint(row, 6, x0_prev, n),
+              "dwm_b200_cfg_dpmpp_step: latents and x0_prev must not overlap each other, pred or row");
+  const unsigned grid = static_cast<unsigned>((n + 255) / 256);
+  cfg_dpmpp_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(pred, cfg, w_uncond, w_cond, n, row,
+                                                                             latents, x0_prev);
   DWM_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -125,6 +125,8 @@ SYMBOLS = {
     "dwm_b200_softmax_rows": (ctypes.c_int, [_p, _i64, _i64, _i64, ctypes.c_float, _p, _i64,
                                             ctypes.c_int, _p]),
     "dwm_b200_lincomb2": (ctypes.c_int, [_p, _p, _p, _p, _i64, _i64, _p, _p]),
+    "dwm_b200_cfg_dpmpp_step": (ctypes.c_int, [_p, ctypes.c_int, ctypes.c_float, ctypes.c_float,
+                                               _i64, _p, _p, _p, _p]),
     "dwm_b200_cfg_ddim_step": (ctypes.c_int, [
         _p, ctypes.c_int, ctypes.c_float, _i64, _i64, _p, ctypes.c_int, _p,
         ctypes.c_int, ctypes.c_float, ctypes.c_int, _p, ctypes.c_int, _p]),

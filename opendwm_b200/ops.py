@@ -875,3 +875,24 @@ def lincomb2(x, y, s0, s1, out):
         x.data_ptr(), y.data_ptr(), s0.data_ptr(), s1.data_ptr(), n, n // s0.numel(),
         out.data_ptr(), _stream()), "dwm_b200_lincomb2")
     return out
+
+
+def cfg_dpmpp_step(pred, latents, x0_prev, row, *, cfg, guidance_scale=1.0):
+    """Fused CFG combine + DPM-Solver++ (midpoint, order <= 2) step, in place on fp32 latents
+    and the x0 history x0_prev (both n elements).  pred: fp32 [cfg * n], unconditional half
+    first; row: fp32 [6] device tensor (c_x, c_m, k_s, k_0, k_1, order).  The CFG weights are
+    fp32(1 - guidance_scale) and fp32(guidance_scale)."""
+    for t, nme in ((pred, "pred"), (latents, "latents"), (x0_prev, "x0_prev"), (row, "row")):
+        _f32(t, nme)
+        if not t.is_contiguous():
+            raise ValueError("cfg_dpmpp_step needs contiguous tensors")
+    n = latents.numel()
+    if cfg not in (1, 2) or pred.numel() != cfg * n or x0_prev.numel() != n or row.numel() != 6:
+        raise ValueError("cfg_dpmpp_step: pred {} must be cfg ({}) x latents {}, x0_prev {} "
+                         "match latents, row {} hold 6 values".format(
+                             pred.numel(), cfg, n, x0_prev.numel(), row.numel()))
+    g = float(guidance_scale)
+    _l.check(_l.load().dwm_b200_cfg_dpmpp_step(
+        pred.data_ptr(), cfg, 1.0 - g, g, n, row.data_ptr(), latents.data_ptr(),
+        x0_prev.data_ptr(), _stream()), "dwm_b200_cfg_dpmpp_step")
+    return latents

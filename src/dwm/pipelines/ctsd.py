@@ -442,11 +442,20 @@ class CrossviewTemporalSD:
         ~600 (UNet) / ~540 (DiT) launches of the step are submitted with one
         cudaGraphLaunch.  The first call per (latents, conditions) pair runs one eager
         warm-up step on a scratch copy (lazy weight packing, condition caches, workspace)
-        and captures."""
-        stateful = not self.is_dit and not hasattr(self.test_scheduler, "final_alpha_cumprod")
+        and captures.
+
+        A multistep scheduler (DPM-Solver++) is captured through its device-state protocol:
+        the step's coefficient row is loaded into the scheduler's static row buffer before
+        each replay and the host counters advance after it; the warm-up step and the capture
+        leave the scheduler as they found it.  A multistep scheduler without that protocol
+        runs eager."""
+        sch = self.test_scheduler
+        multistep = not self.is_dit and not hasattr(sch, "final_alpha_cumprod")
+        device_state = multistep and hasattr(sch, "load_row")
+        stateful = multistep and not device_state
         # sharded steps contain NCCL / symmetric-memory exchanges: captured only on request
         # (DWM_CUDA_GRAPH_SHARDED=1, not yet measured; DiT only, a sharded UNet step always
-        # runs eager); multistep schedulers keep host state
+        # runs eager)
         sharded = self.sharding is not None and (
             not self.is_dit or os.environ.get("DWM_CUDA_GRAPH_SHARDED", "0") != "1")
         if self.sharding is not None and self.sharding.t_ways > 1 and \
@@ -459,37 +468,49 @@ class CrossviewTemporalSD:
             sharded = True          # the same for the view group's cross-view buffers
         if sharded or stateful:
             return self.denoise_step(latents, conditions, idx, timesteps, in_range)
+        # the scheduler's history and row buffers are baked into the graph like the latents
+        sch_bufs = sch.device_state(latents) if device_state else ()
         key = (latents.data_ptr(), tuple(latents.shape), idx is None, in_range is None,
                tuple(sorted((k, v.data_ptr(), tuple(v.shape), v._version)
-                            for k, v in conditions.items() if torch.is_tensor(v))))
+                            for k, v in conditions.items() if torch.is_tensor(v))),
+               tuple(b.data_ptr() for b in sch_bufs))
         graphs = self.__dict__.setdefault("_graphs", {})
         g = graphs.get(key)
         if g is None:
             st = dict(idx=None if idx is None else idx.clone(), ts=timesteps.clone(),
                       rng=None if in_range is None else in_range.clone())
             backup = latents.clone()
+            sch_state = sch.snapshot() if device_state else None
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 self.denoise_step(latents, conditions, st["idx"], st["ts"], st["rng"])
             torch.cuda.current_stream().wait_stream(side)
             latents.copy_(backup)
+            if device_state:
+                sch.restore(sch_state)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 self.denoise_step(latents, conditions, st["idx"], st["ts"], st["rng"])
+            if device_state:
+                sch.restore(sch_state)
             # the entry keeps the keyed tensors alive (addresses are part of the key); a new
             # window / condition set means a new capture, so only the two most recent graphs
             # (and their private memory pools) are kept
             while len(graphs) >= 2:
                 graphs.pop(next(iter(graphs)))
-            g = graphs[key] = (graph, st, (latents, dict(conditions)))
+            g = graphs[key] = (graph, st, (latents, dict(conditions), sch_bufs))
         graph, st = g[:2]
         if idx is not None:
             st["idx"].copy_(idx)
         st["ts"].copy_(timesteps)
         if in_range is not None:
             st["rng"].copy_(in_range)
+        if device_state:
+            sch.load_row()
         graph.replay()
+        if device_state:
+            sch.advance()
         return latents
 
     def _denoise_step_unet(self, latents, conditions, timesteps, do_cfg):
@@ -518,9 +539,14 @@ class CrossviewTemporalSD:
                                device=branch.device, dtype=branch.dtype)
             plan.gather_cfg_tokens(branch, pred)
         sch = self.test_scheduler
+        if hasattr(sch, "cfg_step_"):
+            # DPM-Solver++ multistep (reference :1573-1575, the scheduler counts steps itself):
+            # CFG combine and update in one launch on the latents
+            sch.cfg_step_(pred, latents, self.inference_config.get("guidance_scale", 1),
+                          cfg=2 if do_cfg else 1)
+            return latents
         if not hasattr(sch, "final_alpha_cumprod"):
-            # generic scheduler (e.g. DPM-Solver++ multistep, reference :1573-1575): CFG
-            # combine, then the scheduler's own scalar-timestep step (it counts steps itself)
+            # any other scheduler: CFG combine, then its own scalar-timestep step
             if do_cfg:
                 g = float(self.inference_config.get("guidance_scale", 1))
                 w = self.__dict__.get("_cfg_w")

@@ -7,11 +7,16 @@ src/dwm/pipelines/ctsd.py:981-985, stepped with one scalar timestep per iteratio
 the SD-2.1 `scheduler_config.json`).
 
 All per-step coefficients depend only on the sigma table, so `set_timesteps` evaluates them
-once (fp64 on the host) and keeps them on the device; `step` is then three launches of the
-fused linear-combination kernel (`dwm_b200_lincomb2`) with no host-device traffic:
+once (fp64 on the host) and keeps them on the device; a step is then one launch of the fused
+CFG + DPM-Solver++ kernel (`dwm_b200_cfg_dpmpp_step`) with no host-device traffic:
 
     x0   = c_x[i] * sample + c_m[i] * model_output          (epsilon / sample / v_prediction)
     prev = k_s[i] * sample + k_0[i] * x0_i + k_1[i] * x0_{i-1}
+
+The multistep state the kernel reads is on the device: the x0 history (one buffer, updated in
+place) and, for a captured CUDA graph, the coefficient row and order of the step (`load_row`).
+The host keeps only the counters that pick the row, so a caller that replays a graph loads the
+row before each replay and calls `advance` after it.
 """
 import json
 import math
@@ -68,6 +73,7 @@ class DPMSolverMultistepScheduler:
         self.num_inference_steps = None
         self.timesteps = torch.arange(num_train_timesteps - 1, -1, -1)
         self._begin_index = 0
+        self._x0 = self._row = None       # device x0 history and static coefficient row
 
     @classmethod
     def from_pretrained(cls, pretrained_model_name_or_path, subfolder=None, **kwargs):
@@ -93,7 +99,15 @@ class DPMSolverMultistepScheduler:
 
     def set_begin_index(self, begin_index: int = 0):
         self._begin_index = begin_index
-        self._step_index = begin_index
+        self._reset(begin_index)
+
+    def _reset(self, step_index):
+        """Starts a fresh multistep history at `step_index`: the next step is first order."""
+        self._step_index = step_index
+        self.lower_order_nums = 0
+        for buf in (self._x0, self._row):
+            if buf is not None:
+                buf.zero_()
 
     def set_timesteps(self, num_inference_steps: int, device=None):
         c = self.config
@@ -118,16 +132,17 @@ class DPMSolverMultistepScheduler:
         self.sigmas = torch.from_numpy(sigmas)
         self.timesteps = torch.from_numpy(ts).to(device=device, dtype=torch.int64)
         self.num_inference_steps = n
-        self.model_outputs = [None] * c.solver_order
-        self.lower_order_nums = 0
-        self._step_index = self._begin_index = 0
+        self._begin_index = 0
         self._coef = self._coefficients(sigmas.astype(np.float64)).to(device)
+        self._reset(0)
 
     def _coefficients(self, s):
-        """[n, 2, 5] fp32: for step i and (first-order, second-order) variant the row
-        (c_x, c_m, k_s, k_0, k_1) of the two linear combinations in the module docstring."""
+        """[n, 2, 6] fp32: for step i and (first-order, second-order) variant the row
+        (c_x, c_m, k_s, k_0, k_1, order) of the two linear combinations in the module
+        docstring; the kernel adds the k_1 term exactly when order is 2."""
         n = len(s) - 1
-        out = np.zeros((n, 2, 5))
+        out = np.zeros((n, 2, 6))
+        out[:, 0, 5], out[:, 1, 5] = 1.0, 2.0
         alpha = 1.0 / np.sqrt(s * s + 1.0)
         sig = s * alpha
 
@@ -146,11 +161,11 @@ class DPMSolverMultistepScheduler:
             h = lam(i + 1) - lam(i)
             e1 = math.expm1(-h) if math.isfinite(h) else -1.0      # exp(-h) - 1
             ks, k = sig[i + 1] / sig[i], -alpha[i + 1] * e1
-            out[i, 0] = (cx, cm, ks, k, 0.0)
+            out[i, 0, :5] = (cx, cm, ks, k, 0.0)
             if i > 0:
                 r0 = (lam(i) - lam(i - 1)) / h if math.isfinite(h) else 0.0
-                out[i, 1] = (cx, cm, ks, k * (1.0 + 0.5 / r0), -0.5 * k / r0) if r0 != 0.0 \
-                    else out[i, 0]
+                out[i, 1, :5] = (cx, cm, ks, k * (1.0 + 0.5 / r0), -0.5 * k / r0) if r0 != 0.0 \
+                    else out[i, 0, :5]
         return torch.from_numpy(out.astype(np.float32))
 
     def step(self, model_output, timestep=None, sample=None, generator=None,
@@ -160,37 +175,79 @@ class DPMSolverMultistepScheduler:
                              "'set_timesteps' after creating the scheduler")
         if not model_output.is_cuda:
             raise RuntimeError("scheduler kernels run on CUDA only (no CPU fallback)")
-        i, c = self._step_index, self.config
-        n = len(self.timesteps)
-        lower_final = i == n - 1 and (c.euler_at_final or (c.lower_order_final and n < 15) or
-                                      c.final_sigmas_type == "zero")
-        first = c.solver_order == 1 or self.lower_order_nums < 1 or lower_final
-        if self._coef.device != model_output.device:
-            self._coef = self._coef.to(model_output.device)
-        co = self._coef[i, 0 if first else 1]
-        x = sample.to(torch.float32).contiguous()
-        m = model_output.to(torch.float32).contiguous()
-        x0 = torch.empty_like(x)
-        _ops.lincomb2(x, m, co[0:1], co[1:2], x0)
-        for k in range(c.solver_order - 1):
-            self.model_outputs[k] = self.model_outputs[k + 1]
-        self.model_outputs[-1] = x0
-        prev = torch.empty_like(x)
-        _ops.lincomb2(x, x0, co[2:3], co[3:4], prev)
-        if not first:
-            out = torch.empty_like(x)
-            _ops.lincomb2(prev, self.model_outputs[-2], self._one(x.device), co[4:5], out)
-            prev = out
-        if self.lower_order_nums < c.solver_order:
-            self.lower_order_nums += 1
-        self._step_index += 1
+        prev = torch.empty(sample.shape, device=model_output.device, dtype=torch.float32)
+        prev.copy_(sample)
+        self.cfg_step_(model_output.to(torch.float32).contiguous(), prev, cfg=1)
         prev = prev.to(model_output.dtype)
         if not return_dict:
             return (prev,)
         return SchedulerOutput(prev_sample=prev)
 
-    def _one(self, device):
-        one = self.__dict__.get("_one_t")
-        if one is None or one.device != device:
-            one = self._one_t = torch.ones(1, device=device)
-        return one
+    def cfg_step_(self, pred, latents, guidance_scale=1.0, cfg=2):
+        """One step on fp32 `latents` in place from fp32 `pred` [cfg * latents.numel()]
+        (unconditional half first when cfg is 2): the CFG combine
+        u + guidance_scale * (c - u) and the DPM-Solver++ update in one launch.  Under CUDA-graph
+        capture the launch reads the static row buffer, which the replaying caller fills with
+        `load_row` before each replay (and calls `advance` after it)."""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run "
+                             "'set_timesteps' after creating the scheduler")
+        x0, row = self.device_state(latents)
+        if not torch.cuda.is_current_stream_capturing():
+            i, variant = self._row_index()
+            row = self._coef[i, variant]
+        _ops.cfg_dpmpp_step(pred, latents, x0, row, cfg=cfg, guidance_scale=guidance_scale)
+        self.advance()
+        return latents
+
+    # -- device-state protocol: what a caller replaying the step from a CUDA graph needs ------
+    def device_state(self, sample):
+        """(x0 history, coefficient row) device buffers for steps on `sample`; allocated on
+        first use and kept (a captured graph holds their addresses) until the sample's size or
+        device changes, which is only allowed at the start of a schedule."""
+        dev = sample.device
+        if self._coef.device != dev:
+            self._coef = self._coef.to(dev)
+        if self._row is None or self._row.device != dev:
+            self._row = torch.zeros(6, device=dev)
+        if self._x0 is None or self._x0.device != dev or self._x0.numel() != sample.numel():
+            if self.lower_order_nums > 0:
+                raise ValueError("the sample changed size or device within a schedule; call "
+                                 "set_timesteps or set_begin_index first")
+            self._x0 = torch.zeros(sample.numel(), device=dev)
+        return self._x0, self._row
+
+    def _row_index(self):
+        """Host bookkeeping of the next step: (step index, 0 first / 1 second order)."""
+        i, c = self._step_index, self.config
+        n = len(self.timesteps)
+        if not 0 <= i < n:
+            raise IndexError("step {} is outside the {}-step schedule".format(i, n))
+        lower_final = i == n - 1 and (c.euler_at_final or (c.lower_order_final and n < 15) or
+                                      c.final_sigmas_type == "zero")
+        first = c.solver_order == 1 or self.lower_order_nums < 1 or lower_final
+        return i, 0 if first else 1
+
+    def load_row(self):
+        """Copies the next step's coefficient row and order into the static row buffer."""
+        i, variant = self._row_index()
+        self._row.copy_(self._coef[i, variant])
+
+    def advance(self):
+        """Advances the host counters past one step."""
+        if self.lower_order_nums < self.config.solver_order:
+            self.lower_order_nums += 1
+        self._step_index += 1
+
+    def snapshot(self):
+        """The multistep state (counters, x0 history, row) for `restore`."""
+        return (self._step_index, self.lower_order_nums,
+                None if self._x0 is None else self._x0.clone(),
+                None if self._row is None else self._row.clone())
+
+    def restore(self, state):
+        """Puts back a `snapshot`, in place in the buffers a captured graph reads."""
+        self._step_index, self.lower_order_nums, x0, row = state
+        for buf, old in ((self._x0, x0), (self._row, row)):
+            if buf is not None:
+                buf.copy_(old) if old is not None else buf.zero_()
